@@ -29,6 +29,16 @@ def rand_poly(moduli, N, rng):
     return np.stack([rng.integers(0, int(q), N, dtype=U64) for q in moduli])
 
 
+def launch_delta(fn):
+    """Kernel launches that one call of fn() makes, from the library's launch counter (lgpu_launch_count). An NTT / INTT at
+    N > 2^12 counts 1 for a persistent single-pass launch and 2 for the two-pass kernels, so a test can assert which path
+    a call took."""
+    import lattigo_b200 as lb
+    n0 = lb.lib().lgpu_launch_count()
+    fn()
+    return lb.lib().lgpu_launch_count() - n0
+
+
 def small_poly_rns(coeffs, moduli):
     """Signed small integer coefficients -> RNS rows."""
     return np.stack([np.array([int(c) % int(q) for c in coeffs], dtype=U64) for q in moduli])

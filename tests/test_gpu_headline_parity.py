@@ -32,9 +32,24 @@ def _torch_rand_rows(N, mods, lead, g):
 
 def test_ckks_l44_headline_config_vs_oracle():
     """bench.py's workload (preset CKKS_L44, level 43, beta = 11 digits of 4 limbs, lazy u64 accumulation over 11 terms
-    in K3) bit-exact against the oracle for 2 pairs: device-resident entry point, host-buffer entry point, and batch
-    consistency. Reference op sequence: schemes/ckks/evaluator.go:719-872 + :477-515 over
-    core/rlwe/evaluator_gadget_product.go:129-201."""
+    in K3) bit-exact against the oracle for every pair of a batch of 5 (device-resident entry point), for 2 pairs through
+    the host-buffer entry point, and batch consistency against a single-pair call. At batch 5 the fused ModDown INTT
+    (4 P rows x 5 polynomials per component) and the rescale INTT (the last row) both take the two-pass kernels.
+    Reference op sequence: schemes/ckks/evaluator.go:719-872 + :477-515 over core/rlwe/evaluator_gadget_product.go:129-201."""
+    _ckks_l44_case(5)
+
+
+@pytest.mark.parametrize("batch", [63, 64])
+def test_ckks_l44_headline_persistent_batches_vs_oracle(batch):
+    """The headline case of test_ckks_l44_headline_config_vs_oracle at the batches where its inverse transforms run the
+    persistent kernels: at 63 the ModDown INTT (252 limb-transforms) goes persistent and the rescale INTT (63) stays
+    two-pass, at 64 (the benchmark's shape and sub-batch) both are persistent. Every pair against the oracle; the
+    single-pair call of the batch-consistency check runs the two-pass kernels, so it compares the two paths on the
+    device."""
+    _ckks_l44_case(batch)
+
+
+def _ckks_l44_case(batch):
     import torch
     lb = _lb()
     from lattigo_b200 import params as presets
@@ -50,7 +65,6 @@ def test_ckks_l44_headline_config_vs_oracle():
     evk_t = _torch_rand_rows(N, q + p, (nd, 1, 2), g)
     rlk = lb.GadgetCiphertext(ctx, evk_t, level, levelP)
     ev = lb.CKKSEvaluator(ctx, rlk)
-    batch = 5
     a = _torch_rand_rows(N, q, (batch, 2), g); b = _torch_rand_rows(N, q, (batch, 2), g)
     out = ev.MulRelinRescaleNew(a, b)
     torch.cuda.synchronize()
@@ -58,16 +72,18 @@ def test_ckks_l44_headline_config_vs_oracle():
     assert torch.equal(out[3:4], one)
     params = O.Parameters(logN, q, p)
     ev_o = O.CKKSEvaluator(params, O.GadgetCiphertext(ctx.to_host(evk_t), level + 1, levelP + 1))
-    ah, bh, oh = ctx.to_host(a[:2]), ctx.to_host(b[:2]), ctx.to_host(out[:2])
-    want = np.zeros((2, 2, level, N), dtype=U64)
-    for i in range(2):
+    ah, bh, oh = ctx.to_host(a), ctx.to_host(b), ctx.to_host(out)
+    bad = []
+    for i in range(batch):
         r = ev_o.Rescale(ev_o.MulRelinNew([ah[i, 0], ah[i, 1]], [bh[i, 0], bh[i, 1]]))
-        want[i, 0], want[i, 1] = r
-    assert np.array_equal(oh, want)
-    # host-buffer entry point at the same size (lgpu_ckks_mulrelin_rescale_batch_host, chunked 2-stream pipeline)
+        if not (np.array_equal(oh[i, 0], r[0]) and np.array_equal(oh[i, 1], r[1])):
+            bad.append(i)
+    assert bad == [], "pairs that differ from the oracle: %s" % bad
+    # host-buffer entry point at the same size (lgpu_ckks_mulrelin_rescale_batch_host, chunked 2-stream pipeline), against
+    # the device results just checked
     out_host = np.zeros((2, 2, level, N), dtype=U64)
-    ev.MulRelinRescaleHost(np.ascontiguousarray(ah), np.ascontiguousarray(bh), out_host, chunk=1)
-    assert np.array_equal(out_host, want)
+    ev.MulRelinRescaleHost(np.ascontiguousarray(ah[:2]), np.ascontiguousarray(bh[:2]), out_host, chunk=1)
+    assert np.array_equal(out_host, oh[:2])
     ctx.close()
 
 
@@ -121,20 +137,25 @@ def test_ntt_accepts_words_above_2_52():
     """Ring.NTT ends in a full reduction in the reference (NTTStandard = nttCoreLazy + reducevec, ring/ntt.go:174-177), so
     it accepts lazily accumulated words; the FP64-pipe kernels must not assume inputs below 2^52."""
     lb = _lb()
-    for logN in (12, 16):
+    # (logN, batch, kernel launches): at N = 2^16 one polynomial takes the two-pass kernels (2 launches for the 2 FP64-pipe
+    # rows, 2 for the 56-bit row), 64 polynomials the persistent ones (1 + 1)
+    for logN, batch, launches in ((12, 1, None), (16, 1, 4), (16, 64, 2)):
         N = 1 << logN
         q, p = O.gen_moduli(logN + 1, [56, 45, 45], [55])
         Q = [q[1], q[2], q[0]]
         ctx = lb.Context(logN, Q)
         ring = O.Ring(N, Q)
-        rng = np.random.default_rng(52 + logN)
+        rng = np.random.default_rng(52 + logN + batch)
         # values up to 2^63: the reference's lazy arithmetic does not wrap for 45/56-bit primes there
-        x = rng.integers(0, 1 << 63, (len(Q), N), dtype=U64)
-        x[:, ::7] = rng.integers(0, 1 << 40, (len(Q), (N + 6) // 7), dtype=U64)
-        want = np.empty_like(x); ring.NTT(x, want)
-        d = ctx.to_device(x); o = ctx.ringQ.NewPoly()
-        ctx.ringQ.NTT(d, o)
-        assert np.array_equal(ctx.to_host(o), want), logN
+        x = rng.integers(0, 1 << 63, (batch, len(Q), N), dtype=U64)
+        x[:, :, ::7] = rng.integers(0, 1 << 40, (batch, len(Q), (N + 6) // 7), dtype=U64)
+        want = np.empty_like(x)
+        for b in range(batch):
+            ring.NTT(x[b], want[b])
+        d = ctx.to_device(x); o = ctx.ringQ.NewPoly(batch)
+        n = H.launch_delta(lambda: ctx.ringQ.NTT(d, o))
+        assert launches is None or n == launches, (logN, batch, n)
+        assert np.array_equal(ctx.to_host(o), want), (logN, batch)
         ctx.close()
 
 

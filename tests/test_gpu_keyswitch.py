@@ -366,6 +366,16 @@ def test_ckks_mulrelin_rescale_small_and_host_path():
 def test_ckks_mulrelin_rescale_full_size_pn16qp1761():
     """BASELINE config 3 at full size (N = 2^16, 34 + 4 limbs): bit-exact vs the oracle for 2 ciphertext pairs,
     and batch-consistency (element i of a batch == the same pair evaluated alone) as the size-independent check."""
+    _pn16qp1761_case(batch=6, n_oracle=2)
+
+
+def test_ckks_mulrelin_rescale_full_size_pn16qp1761_batch16():
+    """The same at batch 16, where the ModDown INTT of the 4 P rows runs 64 limb-transforms (the persistent kernels):
+    every pair against the oracle."""
+    _pn16qp1761_case(batch=16, n_oracle=16)
+
+
+def _pn16qp1761_case(batch, n_oracle):
     import torch
     lb = _lb()
     from lattigo_b200 import params as presets
@@ -386,18 +396,18 @@ def test_ckks_mulrelin_rescale_full_size_pn16qp1761():
     evk_t = rand_rows(q + p, (nd, 1, 2))
     rlk = lb.GadgetCiphertext(ctx, evk_t, level, levelP)
     ev = lb.CKKSEvaluator(ctx, rlk)
-    batch = 6
     a = rand_rows(q, (batch, 2)); b = rand_rows(q, (batch, 2))
     out = ev.MulRelinRescaleNew(a, b)
     torch.cuda.synchronize()
     one = ev.MulRelinRescaleNew(a[4:5].contiguous(), b[4:5].contiguous())
     assert torch.equal(out[4:5], one)
-    # oracle on 2 pairs
+    # oracle on the first n_oracle pairs
     params = O.Parameters(logN, q, p)
     rlk_o = O.GadgetCiphertext(ctx.to_host(evk_t), level + 1, levelP + 1)
     ev_o = O.CKKSEvaluator(params, rlk_o)
-    ah, bh, oh = ctx.to_host(a[:2]), ctx.to_host(b[:2]), ctx.to_host(out[:2])
-    for i in range(2):
+    n = n_oracle
+    ah, bh, oh = ctx.to_host(a[:n]), ctx.to_host(b[:n]), ctx.to_host(out[:n])
+    for i in range(n):
         r = ev_o.Rescale(ev_o.MulRelinNew([ah[i, 0], ah[i, 1]], [bh[i, 0], bh[i, 1]]))
         assert np.array_equal(oh[i, 0], r[0]) and np.array_equal(oh[i, 1], r[1]), i
     ctx.close()
@@ -431,6 +441,17 @@ def test_ringqp_dispatch(small):
 def test_bgv_rotate_full_size_n15qp880():
     """BASELINE config 4 shape: BGV N15QP880 RotateColumns = Evaluator.Automorphism (key-switch + NTT-domain
     permutation), batch of ciphertexts, bit-exact vs the oracle for 2 of them + batch consistency."""
+    _bgv_n15qp880_rotate_case(batch=5, n_oracle=2)
+
+
+def test_bgv_rotate_full_size_n15qp880_batch16():
+    """The same at batch 16, every ciphertext against the oracle: the ModDown INTT of the 4 P rows runs 64
+    limb-transforms of 47-bit primes at N = 2^15, the persistent integer inverse without lazy corrections
+    (IntInvOps<3, 2>), which no other preset selects."""
+    _bgv_n15qp880_rotate_case(batch=16, n_oracle=16)
+
+
+def _bgv_n15qp880_rotate_case(batch, n_oracle):
     import torch
     lb = _lb()
     from lattigo_b200 import params as presets
@@ -453,7 +474,6 @@ def test_bgv_rotate_full_size_n15qp880():
     ev = lb.Evaluator(ctx)
     params = O.Parameters(logN, q, p)
     galEl = params.GaloisElement(3)
-    batch = 5
     ct = rand_rows(q, (batch, 2))
     out = torch.zeros_like(ct)
     ev.Automorphism(ct, galEl, gk, out)
@@ -462,8 +482,9 @@ def test_bgv_rotate_full_size_n15qp880():
     assert torch.equal(out[3:4], one)
     gk_o = O.GadgetCiphertext(ctx.to_host(gk_t), level + 1, levelP + 1)
     ev_o = O.Evaluator(params)
-    cth, oh = ctx.to_host(ct[:2]), ctx.to_host(out[:2])
-    for i in range(2):
+    n = n_oracle
+    cth, oh = ctx.to_host(ct[:n]), ctx.to_host(out[:n])
+    for i in range(n):
         w = [np.zeros((level + 1, N), dtype=U64) for _ in range(2)]
         ev_o.Automorphism([cth[i, 0], cth[i, 1]], galEl, gk_o, w)
         assert np.array_equal(oh[i, 0], w[0]) and np.array_equal(oh[i, 1], w[1]), i
