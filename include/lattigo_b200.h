@@ -385,6 +385,26 @@ int lgpu_ckks_mulrelin_rescale_batch(lgpu_ctx* ctx, int level, const uint64_t* c
 int lgpu_ckks_mulrelin_rescale_batch_host(lgpu_ctx* ctx, int level, const uint64_t* ct_a_host, const uint64_t* ct_b_host,
                                           const lgpu_gadget_ct* rlk, int nb_rescales, uint64_t* ct_out_host, int batch, int chunk);
 
+/* ---- BGV / BFV ciphertext multiplication (schemes/bgv) ---------------------------------------------------------
+ * State of bgv.NewParameters' ringQMul + newEvaluatorPrecomp (schemes/bgv/params.go:98-109, evaluator.go:38-70) for the
+ * context's Q: the plaintext modulus t, tMontgomery, levelQMul[] and the Q <-> QMul basis extender.
+ * qmul: the caller's RingQMul moduli (as lgpu_create takes Q and P), in the reference's
+ * NextDownstreamPrimes(61, NthRoot) order. Errors: t < 2, t >= q_0, t in Q, a QMul prime in Q,
+ * nqmul < levelQMul[MaxLevel] + 1, a ConjugateInvariant ctx. A host-only ctx (device < 0) gives a host-only handle (argument
+ * checks, no device execution). Destroy before ctx. */
+typedef struct lgpu_bgv lgpu_bgv;
+int lgpu_bgv_create(lgpu_ctx* ctx, uint64_t t, const uint64_t* qmul, int nqmul, lgpu_bgv** out);
+void lgpu_bgv_destroy(lgpu_bgv* ev);
+/* bgv.Evaluator.MulRelin of two degree-1 ciphertexts followed by nb_rescales x Rescale (scale_invariant = 0;
+ * evaluator.go:529-556, tensorStandard :592-667, Rescale :1363-1393), or MulRelinScaleInvariant (scale_invariant = 1, BFV;
+ * :806-864, tensorScaleInvariant :898-1070; nb_rescales must be 0). ct_a, ct_b: [batch][2][level+1][N], NTT domain;
+ * ct_out: [batch][2][level+1-nb_rescales][N]. ct_a == ct_b is the squaring case. ct_out == ct_a is allowed when
+ * nb_rescales == 0; no other overlap. rlk: the relinearization key of ctx's (Q, P).
+ * Scale bookkeeping stays with the caller: the reference sets the output scale to s_a * s_b (BGV), divided by q_level for
+ * each Rescale, and to MulScaleInvariant(s_a, s_b, level) = s_a * s_b / (-Q_level mod t) for BFV (:983-989). */
+int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const uint64_t* ct_b, const lgpu_gadget_ct* rlk,
+                            int scale_invariant, int nb_rescales, uint64_t* ct_out, int batch, void* stream);
+
 
 /* ---- launch accounting / profiling (used by bench.py) ------------------------------------------------------- */
 enum lgpu_kclass {

@@ -7,6 +7,7 @@ from .ring import Context, Ring, SubRing, OPS, OP  # noqa: F401
 from .rlwe import (GadgetCiphertext, BasisExtender, Decomposer, Evaluator, CKKSEvaluator, div_by_last_modulus_many,  # noqa: F401
                    automorphism_ntt_index, automorphism_ntt_with_index, automorphism_ntt, automorphism)
 from .ringqp import RingQP, Poly as PolyQP  # noqa: F401
+from .bgv import BGVEvaluator  # noqa: F401
 from . import lintrans  # noqa: F401,E402
 from . import wire  # noqa: F401,E402
 from . import rgsw  # noqa: F401,E402

@@ -80,6 +80,9 @@ def lib():
             "lgpu_evaluator_relinearize": [vp, i, vp, vp, vp, i, vp],
             "lgpu_ckks_mulrelin_rescale_batch": [vp, i, vp, vp, vp, i, vp, i, vp],
             "lgpu_ckks_mulrelin_rescale_batch_host": [vp, i, vp, vp, vp, i, vp, i, i],
+            "lgpu_bgv_create": [vp, u64, vp, i, c.POINTER(vp)],
+            "lgpu_bgv_destroy": [vp],
+            "lgpu_bgv_mulrelin_batch": [vp, i, vp, vp, vp, i, i, vp, i, vp],
             "lgpu_lintrans_evaluate_many": [vp, i, vp, vp, i, vp, vp, vp, i, vp],
             "lgpu_evaluator_automorphism_hoisted_lazy": [vp, i, vp, vp, i, u64, vp, vp, vp, vp, vp, i, z, z, z, vp],
             "lgpu_rgsw_external_product": [vp, vp, i, vp, vp, vp, i, i, vp],
@@ -102,9 +105,10 @@ def lib():
         for name, args in sig.items():
             f = getattr(L, name)
             f.argtypes = args
-            if name != "lgpu_destroy":
+            if name not in ("lgpu_destroy", "lgpu_bgv_destroy"):
                 f.restype = i
         L.lgpu_destroy.restype = None
+        L.lgpu_bgv_destroy.restype = None
         L.lgpu_galois_element.restype = c.c_uint64
         L.lgpu_galois_element.argtypes = [vp, c.c_longlong]
         L.lgpu_launch_count.restype = c.c_ulonglong

@@ -467,7 +467,7 @@ static int gadget_product_single_p_lazy(const Ctx* c, int levelQ, CSpan cx, cons
     return 0;
 }
 
-static int check_evk(const Ctx* c, int levelQ, const GadgetCt& evk) {
+int check_evk(const Ctx* c, int levelQ, const GadgetCt& evk) {
     if (!evk.data) { set_error("null evaluation key"); return -1; }
     if (evk.levelQ < 0 || evk.levelQ >= c->nQ || evk.levelP < -1 || evk.levelP >= c->nP) { set_error("evaluation key levels out of range"); return -1; }
     if (levelQ < 0 || levelQ > evk.levelQ) { set_error("levelQ out of range for this evaluation key"); return -1; }
@@ -715,7 +715,7 @@ static int ckks_mulrelin_rescale_chunk(const Ctx* c, int level, const u64* ctA, 
 // Sub-batches bound the key-switch scratch (P1 is 270 MB per ciphertext at L = 44: 17 GB for 64) while the evaluation key is streamed
 // once per sub-batch. H100 (700 W), L = 44, batch 64: 1 264 ct/s with sub-batches of 32, 1 271 with 64 (profiles/h100_switch_ab.md).
 // LGPU_BATCH_CHUNK overrides the default.
-static int batch_chunk() {
+int batch_chunk() {
     static int v = [] {
         const char* e = getenv("LGPU_BATCH_CHUNK");
         int x = e ? atoi(e) : 64;
@@ -751,8 +751,6 @@ static int ckks_mulrelin_rescale_chunk(const Ctx* c, int level, const u64* ctA, 
     u64* d0 = buf.p;
     u64* d1 = d0 + (size_t)batch * nq * N;
     u64* d2 = d1 + (size_t)batch * nq * N;
-    u64* t0 = d2 + (size_t)batch * nq * N;
-    u64* t1 = t0 + (size_t)batch * nq * N;
     {
         TensorParams p;
         p.limbs = c->d_limbs;
@@ -763,6 +761,20 @@ static int ckks_mulrelin_rescale_chunk(const Ctx* c, int level, const u64* ctA, 
         ckks_tensor_kernel<<<grid, 256, 0, st>>>(p);
         LGPU_CUDA_OK(cudaGetLastError());
     }
+    return mulrelin_tail(c, level, buf.p, rlk, nb_rescales, out, batch, st);
+}
+
+// The relinearization (+ rescale) that follows every degree-1 x degree-1 tensor: out = (d0, d1) + GadgetProduct(d2, rlk), then
+// nb_rescales x DivRoundByLastModulusNTT. d: five consecutive [batch][level+1][N] blocks d0, d1, d2 (canonical, NTT domain) and the
+// scratch t0, t1; d0 and d1 are overwritten.
+int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_rescales, u64* out, int batch, cudaStream_t st) {
+    const size_t N = c->N, nq = level + 1;
+    const size_t ct_stride = 2 * nq * N;
+    u64* d0 = d;
+    u64* d1 = d0 + (size_t)batch * nq * N;
+    u64* d2 = d1 + (size_t)batch * nq * N;
+    u64* t0 = d2 + (size_t)batch * nq * N;
+    u64* t1 = t0 + (size_t)batch * nq * N;
     if (rlk.levelP >= 1 && rlk.pw2 == 0 && fz_applicable(c, level, rlk.levelP) && (nb_rescales == 0 || (nb_rescales == 1 && level >= 1))) {
         // fused tail: accumulators -> (ModDown + add of d0/d1) in one chunk-pass epilogue -> fused rescale
         const size_t np = rlk.levelP + 1;

@@ -83,5 +83,9 @@ int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs,
 
 int ckks_mulrelin_rescale(const Ctx* c, int level, const u64* ctA, const u64* ctB, const GadgetCt& rlk, int nb_rescales, u64* out, int batch,
                           cudaStream_t st);
+// shared by the CKKS and BGV/BFV multiplications (composite.cu, bgv.cu)
+int check_evk(const Ctx* c, int levelQ, const GadgetCt& evk);
+int batch_chunk();
+int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_rescales, u64* out, int batch, cudaStream_t st);
 
 }  // namespace lgpu

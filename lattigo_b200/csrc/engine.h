@@ -135,7 +135,8 @@ u64 h_powmod(u64 a, u64 e, u64 m);
 u64 h_invmod(u64 a, u64 m);  // m prime
 bool h_is_prime(u64 n);
 u64 h_mform(u64 a, u64 q);   // a * 2^64 mod q
-int build_context(Ctx* c, int device, int logN, int ring_type, const u64* q, int nq, const u64* p, int np);
+// decomposer = false skips the Decomposer constant sets (a context that never key-switches)
+int build_context(Ctx* c, int device, int logN, int ring_type, const u64* q, int nq, const u64* p, int np, bool decomposer = true);
 void destroy_context(Ctx* c);
 int ensure_scratch(Ctx* c, size_t words);
 // (re)derives the fast-path tables of global limb g from its Montgomery root tables and uploads them

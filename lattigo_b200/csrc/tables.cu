@@ -262,7 +262,7 @@ int upload_limb_tables(Ctx* c, int i) {
     return 0;
 }
 
-int build_context(Ctx* c, int device, int logN, int ring_type, const u64* q, int nq, const u64* p, int np) {
+int build_context(Ctx* c, int device, int logN, int ring_type, const u64* q, int nq, const u64* p, int np, bool decomposer) {
     if (logN < 4 || logN > 17) { set_error("invalid ring degree: need 16 <= N <= 2^17"); return -1; }
     if (nq <= 0 || !q) { set_error("invalid ModuliChain (must be non-empty)"); return -1; }
     if (nq + np > kMaxRows) { set_error("too many moduli"); return -1; }
@@ -324,7 +324,7 @@ int build_context(Ctx* c, int device, int logN, int ring_type, const u64* q, int
         }
         // Decomposer, ring/basis_extension.go:333-373
         c->muc_dec.clear();
-        for (int lvlP = 0; lvlP < np - 1; lvlP++) {
+        for (int lvlP = 0; decomposer && lvlP < np - 1; lvlP++) {
             const int nbPi = lvlP + 2;
             const int ndig = (nq + nbPi - 1) / nbPi;
             std::vector<std::vector<ModUpSet>> per_digit(ndig);

@@ -9,6 +9,8 @@ produces the per-config table that DESIGN.md quotes and writes it as JSON (defau
       lgpu_ntt_then_mul_coeffs_montgomery
   C3  CKKS PN16QP1761, batch 64 pairs at level 33: MulRelin + Rescale, ct/s
   C4  BGV N15QP880, batch 128 at level 19: one Galois rotation (Evaluator.Automorphism), ct/s
+  C4mul  the same ciphertexts: BGV MulRelin + Rescale and BFV MulRelinScaleInvariant (lgpu_bgv_mulrelin_batch), ct/s;
+         algorithmic bytes 4*S(20) in + 2*S(19) (BGV) or 2*S(20) (BFV) out per pair + the relinearization key once per batch
 """
 import argparse
 import json
@@ -35,6 +37,17 @@ def timeit(fn, iters, warmup, flush):
         torch.cuda.synchronize()
         ts.append(a.elapsed_time(b) * 1e-3)
     return float(np.median(ts)), float(np.min(ts))
+
+
+def power_limit_w():
+    """Enforced power limit of GPU 0 (read-only nvidia-smi query), or None where it cannot be read."""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        return None
 
 
 def rand_rows(moduli, N, batch, rng, dev):
@@ -64,7 +77,8 @@ def main():
     torch.cuda.set_device(0)
     rng = np.random.default_rng(20260922)
     flush = torch.zeros(256 << 20, dtype=torch.uint8, device=dev)   # 256 MiB > the 126 MB L2
-    res = {"gpu": torch.cuda.get_device_name(0), "timing": "cuda events, median of %d, L2 flushed before every iteration" % args.iters}
+    res = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": power_limit_w(),
+           "timing": "cuda events, median of %d, L2 flushed before every iteration" % args.iters}
     want = set(args.only.split(",")) if args.only else None
 
     def on(name):
@@ -136,6 +150,26 @@ def main():
         alg = batch * 4 * Sl(level + 1) + gk.struct.n_digits * 2 * Sl(level + 1 + levelP + 1) + ctx.N * 8
         res["C4"] = {"workload": "BGV N15QP880, batch 128 at level 19: Evaluator.Automorphism (rotate by 1)", "ms_per_batch": med * 1e3,
                      "ct_per_s": batch / med, "alg_bytes_per_batch": alg, "alg_GBs": alg / med / 1e9}
+        ctx.close()
+
+    if on("C4mul"):
+        P = presets.PRESETS["BGV_N15QP880"]
+        ctx = lb.Context(15, P["Q"], P["P"])
+        level, levelP, batch = len(P["Q"]) - 1, len(P["P"]) - 1, 128
+        rlk = lb.GadgetCiphertext(ctx, rand_evk(ctx, level, levelP, rng, dev), level, levelP)
+        a = rand_rows(ctx.Q, ctx.N, batch * 2, rng, dev).view(batch, 2, level + 1, ctx.N)
+        b = rand_rows(ctx.Q, ctx.N, batch * 2, rng, dev).view(batch, 2, level + 1, ctx.N)
+        Sl = lambda l: l * ctx.N * 8
+        key = rlk.struct.n_digits * 2 * Sl(level + 1 + levelP + 1)
+        for name, si, out_limbs in (("C4mul_bgv", False, level), ("C4mul_bfv", True, level + 1)):
+            ev = lb.BGVEvaluator(ctx, P["T"], P["QMul"], rlk, scale_invariant=si)
+            fn = (lambda: ev.MulRelinNew(a, b)) if si else (lambda: ev.MulRelinRescaleNew(a, b))
+            med, mn = timeit(fn, args.iters, 3, flush)
+            alg = batch * (4 * Sl(level + 1) + 2 * Sl(out_limbs)) + key
+            res[name] = {"workload": "BGV N15QP880 (t = 65537, 12 QMul primes), batch 128 pairs at level 19: "
+                         + ("MulRelinScaleInvariant (BFV)" if si else "MulRelin + Rescale (BGV)"),
+                         "ms_per_batch": med * 1e3, "ct_per_s": batch / med, "alg_bytes_per_batch": alg, "alg_GBs": alg / med / 1e9}
+            ev.close()
         ctx.close()
 
     if on("BOOT"):
