@@ -298,6 +298,27 @@ int lgpu_evaluator_automorphism_hoisted_lazy(lgpu_ctx* ctx, int level_q, const u
                                              uint64_t gal_el, const lgpu_gadget_ct* gk, uint64_t* out0q, uint64_t* out0p, uint64_t* out1q,
                                              uint64_t* out1p, int batch, size_t stride_ct, size_t stride_q, size_t stride_p, void* stream);
 
+/* ---- slot aggregation (core/rlwe/inner_sum.go), Standard ring only -------------------------------------------------------
+ * Evaluator.PartialTracesSum (:147-292): ct_out = sum_{i<n} phi(i * offset)(ct_in), phi(k) = Automorphism by GaloisElement(k), with
+ * the reference's schedule: log2(n) + HW(n) - 1 key switches, one DecomposeNTT per doubling step, the terms of the non-power-of-two
+ * bits accumulated mod QP and divided by P once. InnerSum / RotateAndAdd: offset = batchSize; Replicate: offset = -batchSize.
+ * ct_in, ct_out: [batch][2][level+1][N]; is_ntt = 0: coefficient domain in and out (with n = 1 the output is INTT(ct_in), as the
+ * reference's copy followed by its trailing INTT). ct_out == ct_in allowed, no other overlap.
+ * Errors: n <= 0 or offset == 0 ("partialtrace: invalid parameter (n = 0 or batchSize = 0)"), a ConjugateInvariant ctx, n >= 2
+ * without a P ring, a key with levelP != MaxLevelP or BaseTwoDecomposition != 0, a missing key ("GaloisKey[g] is missing").
+ * Unlike the reference, which fails at the first missing key after part of the work, every key is checked before any device work;
+ * the argument checks also run on a host-only ctx. */
+int lgpu_evaluator_partial_traces_sum(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int is_ntt, int offset, int n,
+                                      const lgpu_galois_keys* gks, uint64_t* ct_out, int batch, void* stream);
+/* Evaluator.Trace (:36-116), 0 <= log_n <= LogN - 1: keeps the plaintext coefficients whose index is a multiple of
+ * gap = 2^(LogN - log_n - 1) (gap = N for log_n = 0) and zeroes the others; gap = 1 is a copy. ct_in: [batch][2][level_in+1][N],
+ * ct_out: [batch][2][level_out+1][N]; the result is at level min(level_in, level_out) and rows 0..that level of each component are
+ * written, the block keeps its layout (as in lgpu_lintrans_evaluate_many). ct_out == ct_in allowed (with level_out == level_in).
+ * Keys: GaloisElement(2^i) for log_n <= i < LogN - 1, and NthRoot - 1 for log_n = 0, with a P ring and BaseTwoDecomposition = 0;
+ * errors as for lgpu_evaluator_partial_traces_sum, checked before any device work. */
+int lgpu_evaluator_trace(lgpu_ctx* ctx, int level_in, const uint64_t* ct_in, int is_ntt, int log_n, const lgpu_galois_keys* gks,
+                         uint64_t* ct_out, int level_out, int batch, void* stream);
+
 /* ---- RGSW (core/rgsw) --------------------------------------------------------------------------------------------------
  * rgsw.Evaluator.ExternalProduct (core/rgsw/evaluator.go:39-88): RLWE x RGSW -> RLWE at the RGSW ciphertext's levels.
  * rgsw0 / rgsw1 = rgsw.Ciphertext.Value[0] / Value[1] (core/rgsw/elements.go:11-13). ct_in: [batch][2][level_in+1][N], NTT domain;

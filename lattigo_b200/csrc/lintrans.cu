@@ -106,7 +106,8 @@ __global__ void __launch_bounds__(256) lt_perm_mac_kernel(LtPermMacParams p) {
 // index[j]. In the bit-reversed NTT layout an automorphism maps every aligned block of 2^k coefficients onto an aligned block (multiplication by
 // an odd Galois element preserves the low bits that select the block), so a warp's 32 gathered 8-byte reads cover exactly one 256-byte block:
 // the gather costs no extra sectors, and the separate MAC passes (accumulators re-read and re-written per digit) and permutation passes go away.
-// index == nullptr: no permutation (the plain hoisted product).
+// index == nullptr: no permutation (the plain hoisted product). Acc: accumulate into the outputs, out = CRed(out + v) on every row (the
+// ringqp.Ring.Add that follows AutomorphismHoistedLazy in PartialTracesSum, core/rlwe/inner_sum.go:243-247).
 struct HoistParams {
     const LimbConst* limbs;
     const u64* decomp; size_t d_ds, d_bs; int d_pshift;   // [digit][batch][nqd + np][N]; P rows start d_pshift rows after row nq
@@ -117,6 +118,7 @@ struct HoistParams {
     int nq, np, nQfull, nd, n, batch;
 };
 constexpr int kHoistB = 4;   // batch elements per thread: the key words are loaded once for all of them
+template <bool Acc>
 __global__ void __launch_bounds__(256) lt_hoisted_auto_kernel(HoistParams p) {
     const int r = blockIdx.y;
     const bool isP = r >= p.nq;
@@ -153,8 +155,10 @@ __global__ void __launch_bounds__(256) lt_hoisted_auto_kernel(HoistParams p) {
                 u64 v0 = cred(a0[t], q);
                 if (p.ct0P && !isP) v0 = cred(v0 + p.ct0P[(size_t)(b0 + t) * p.c_bs + (size_t)r * p.n + src], q);
                 const size_t o = (size_t)(b0 + t) * p.o_bs + (size_t)r * p.n + j;
+                u64 v1 = cred(a1[t], q);
+                if (Acc) { v0 = cred(p.out0[o] + v0, q); v1 = cred(p.out1[o] + v1, q); }
                 p.out0[o] = v0;
-                p.out1[o] = cred(a1[t], q);
+                p.out1[o] = v1;
             }
         }
     }
@@ -200,7 +204,7 @@ static std::vector<u64> p_mod_q_mont(const Ctx* c, int levelQ, int levelP) {
 
 // Evaluator.AutomorphismHoistedLazy (core/rlwe/evaluator_automorphism.go:107-165), NTT-domain branch: out = pi_galEl(
 // <decomp, gk> + (P * ct0, 0)) mod QP. ct0P = P * ct0 (rows [0, levelQ], canonical).
-static int check_gk(const Ctx* c, int levelQ, const GadgetCt& gk) {
+int check_gk(const Ctx* c, int levelQ, const GadgetCt& gk) {
     if (!gk.data || gk.levelQ < levelQ || gk.levelQ >= c->nQ || gk.levelP < 0 || gk.levelP >= c->nP) { set_error("Galois key levels out of range"); return -1; }
     if (gk.pw2 != 0) { set_error("method is unsupported for BaseTwoDecomposition != 0"); return -1; }
     if (gk.ndigits < base_rns_decomposition_vector_size(levelQ, gk.levelP)) { set_error("Galois key has too few digits"); return -1; }
@@ -208,7 +212,7 @@ static int check_gk(const Ctx* c, int levelQ, const GadgetCt& gk) {
 }
 
 int automorphism_hoisted_lazy(const Ctx* c, int levelQ, CSpan ct0P, const u64* decomp, int decomp_levelQ, u64 galEl, const GadgetCt& gk,
-                              const AccSpans& out, int batch, cudaStream_t st) {
+                              const AccSpans& out, int batch, cudaStream_t st, bool accumulate) {
     const int levelP = gk.levelP;
     if (levelP < 0) { set_error("AutomorphismHoistedLazy requires a P ring"); return -1; }
     if (check_gk(c, levelQ, gk)) return -1;
@@ -228,13 +232,17 @@ int automorphism_hoisted_lazy(const Ctx* c, int levelQ, CSpan ct0P, const u64* d
         p.ct0P = ct0P.p; p.c_bs = ct0P.batch_stride;
         p.out0 = out.q[0].p; p.out1 = out.q[1].p; p.o_bs = out.q[0].batch_stride;
         p.index = ib.p; p.nq = (int)nq; p.np = (int)np; p.nQfull = c->nQ; p.nd = base_rns_decomposition_vector_size(levelQ, levelP); p.n = c->N; p.batch = batch;
-        // decomposition once, key once per group of kHoistB ciphertexts, P * ct0 on the Q rows, two outputs
-        ProfScope ps(LGPU_KCLASS_MAC, st, 8.0 * N * ((double)(nq + np) * (p.nd * (batch + 2.0 * ((batch + kHoistB - 1) / kHoistB)) + 2.0 * batch) + (double)nq * batch), 1);
+        // decomposition once, key once per group of kHoistB ciphertexts, P * ct0 on the Q rows, two outputs (read back too when accumulating)
+        ProfScope ps(LGPU_KCLASS_MAC, st, 8.0 * N * ((double)(nq + np) * (p.nd * (batch + 2.0 * ((batch + kHoistB - 1) / kHoistB)) + (accumulate ? 4.0 : 2.0) * batch) +
+                                                     (double)nq * batch), 1);
         const int zb = std::max(1, std::min(16, (batch + kHoistB - 1) / kHoistB));
-        lt_hoisted_auto_kernel<<<dim3((c->N + 255) / 256, (unsigned)(nq + np), zb), 256, 0, st>>>(p);
+        const dim3 grid((c->N + 255) / 256, (unsigned)(nq + np), zb);
+        if (accumulate) lt_hoisted_auto_kernel<true><<<grid, 256, 0, st>>>(p);
+        else lt_hoisted_auto_kernel<false><<<grid, 256, 0, st>>>(p);
         LGPU_CUDA_OK(cudaGetLastError());
         return 0;
     }
+    if (accumulate) { set_error("AutomorphismHoistedLazy: accumulation needs QP-stacked outputs"); return -1; }
     Scratch buf;
     if (buf.alloc((size_t)2 * batch * (nq + np) * N + N, st)) return -1;
     AccSpans acc = stacked_acc(buf.p, nq, np, N, batch);

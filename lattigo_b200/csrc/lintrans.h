@@ -20,8 +20,11 @@ struct GaloisKeySet {        // the GaloisKeys map of rlwe.MemEvaluationKeySet, 
 
 u64 galois_element(const Ctx* c, long long k);
 void bsgs_index(const LinTransView& m, std::map<int, std::vector<int>>& index, std::vector<int>& rotN1, std::vector<int>& rotN2);
+// accumulate: out = CRed(out + result) (needs QP-stacked outputs: out.p[k] right after the nq rows of out.q[k], one batch stride)
 int automorphism_hoisted_lazy(const Ctx* c, int levelQ, CSpan ct0P, const u64* decomp, int decomp_levelQ, u64 galEl, const GadgetCt& gk,
-                              const AccSpans& out, int batch, cudaStream_t st);
+                              const AccSpans& out, int batch, cudaStream_t st, bool accumulate = false);
+// Galois key usable by the hoisted products at levelQ: levels in range, BaseTwoDecomposition = 0, enough digits (error set otherwise)
+int check_gk(const Ctx* c, int levelQ, const GadgetCt& gk);
 int lintrans_evaluate_many(const Ctx* c, int level_in, const u64* ct_in, const LinTransView* mats, int n_mats, const GaloisKeySet& gks,
                            u64* const* outs, int* out_levels, int batch, cudaStream_t st);
 

@@ -11,6 +11,14 @@ produces the per-config table that DESIGN.md quotes and writes it as JSON (defau
   C4  BGV N15QP880, batch 128 at level 19: one Galois rotation (Evaluator.Automorphism), ct/s
   C4mul  the same ciphertexts: BGV MulRelin + Rescale and BFV MulRelinScaleInvariant (lgpu_bgv_mulrelin_batch), ct/s;
          algorithmic bytes 4*S(20) in + 2*S(19) (BGV) or 2*S(20) (BFV) out per pair + the relinearization key once per batch
+  C4sum  the same ciphertexts: bgv.Evaluator.InnerSum(batchSize = 1, n = N) -- the n * batchSize == Slots() rule,
+         PartialTracesSum(1, N/2) (14 key switches) + RotateRows + Add -- through lgpu_evaluator_partial_traces_sum, ct/s
+  C3sum  PN16QP1761 batch 64 at level 33: RotateAndAdd(batchSize = 1, n = 7) = PartialTracesSum(1, 7) (4 key switches, two of them
+         lazy QP terms; InnerSum rejects n * batchSize = 7), ct/s
+  C3sum / C4sum also time the same schedule composed from the existing entry points (lgpu_decompose_ntt,
+  lgpu_evaluator_automorphism_hoisted_lazy, lgpu_evaluator_automorphism with the hoisted decomposition, vecops, ModDown) in the
+  same run, and report the kernel launches of one call. Algorithmic bytes: every input and output ciphertext once plus every
+  Galois key once.
 """
 import argparse
 import json
@@ -65,6 +73,123 @@ def rand_evk(ctx, levelQ, levelP, rng, dev):
     for i, q in enumerate(mods):
         data[:, :, :, i] = torch.from_numpy(rng.integers(0, q, size=(nd, 1, 2, ctx.N), dtype=np.uint64).view(np.int64)).to(dev)
     return data
+
+
+def _pts_schedule(ctx, offset, n):
+    """PartialTracesSum's key switches (core/rlwe/inner_sum.go:217-283): per iteration below the top bit of n, the lazy term's
+    rotation (or None) and the doubling rotation."""
+    out = []
+    i, j = 0, n
+    while j > 1:
+        out.append(((n - (n & ((2 << i) - 1))) * offset if j & 1 else None, (1 << i) * offset))
+        i, j = i + 1, j >> 1
+    return out
+
+
+def composed_pts(ctx, rl, keys, ct, offset, n, out):
+    """PartialTracesSum(ct, offset, n), NTT domain, built from the existing entry points: what a caller without the fused call
+    does. Lazy terms use the one-pass QP-stacked AutomorphismHoistedLazy, doublings Evaluator.Automorphism with the hoisted
+    decomposition, then vecop adds and one ModDown."""
+    import ctypes
+    L = lb.lib()
+    b, _, nq, N = ct.shape
+    level, levelP = nq - 1, len(ctx.P) - 1
+    np_ = levelP + 1
+    vp = ctypes.c_void_p
+    gal = lambda k: pow(5, k & (2 * N - 1), 2 * N)
+    st = lb.ring._stream()
+    ADD = lb.OP["Add"]
+    x = ct.clone()
+    tmp = torch.empty_like(x)
+    acc = torch.empty((2, b, nq + np_, N), dtype=torch.int64, device=ct.device)
+    cqp = torch.empty_like(acc)
+    dec = torch.empty((rl.BaseRNSDecompositionVectorSize(level, levelP), b, nq + np_, N), dtype=torch.int64, device=ct.device)
+    W = 8 * N
+    first = True
+    for lazy, dbl in _pts_schedule(ctx, offset, n):
+        lb._lib.check(L.lgpu_decompose_ntt(ctx.h, level, levelP, levelP + 1, vp(x.data_ptr() + nq * W), 1, vp(dec.data_ptr()), b, 2 * nq * N, st))
+        if lazy is not None:
+            base = (acc if first else cqp).data_ptr()
+            lb._lib.check(L.lgpu_evaluator_automorphism_hoisted_lazy(
+                ctx.h, level, vp(x.data_ptr()), vp(dec.data_ptr()), level, gal(lazy), keys[gal(lazy)].ref(), vp(base), vp(base + nq * W),
+                vp(base + b * (nq + np_) * W), vp(base + (b * (nq + np_) + nq) * W), b, 2 * nq * N, (nq + np_) * N, (nq + np_) * N, st))
+            if not first:          # ringQP.Add(accQP, cQP, accQP) on both components
+                for ring, lvl, off in ((lb.ring.RING_Q, level, 0), (lb.ring.RING_P, levelP, nq * W)):
+                    pa, pc = vp(acc.data_ptr() + off), vp(cqp.data_ptr() + off)
+                    lb._lib.check(L.lgpu_vecop(ctx.h, ring, lvl, ADD, pa, pc, pa, None, None, 2 * b, (nq + np_) * N, st))
+            first = False
+        rl.Automorphism(x, gal(dbl), keys[gal(dbl)], tmp, decomp=dec)
+        ringQ = ctx.ringQ.AtLevel(level)
+        ringQ.Add(x.view(-1, nq, N), tmp.view(-1, nq, N), x.view(-1, nq, N))
+    if n & (n - 1):
+        a = acc.data_ptr()
+        lb._lib.check(L.lgpu_evaluator_moddown(ctx.h, level, levelP, vp(a), vp(a + nq * W), vp(a + b * (nq + np_) * W), vp(a + (b * (nq + np_) + nq) * W),
+                                               vp(tmp.data_ptr()), vp(tmp.data_ptr() + nq * W), b, (nq + np_) * N, (nq + np_) * N, 2 * nq * N, st))
+        ctx.ringQ.AtLevel(level).Add(tmp.view(-1, nq, N), x.view(-1, nq, N), out.view(-1, nq, N))
+    else:
+        out.copy_(x)
+
+
+def bench_innersum(name, iters, rng, dev, flush):
+    if name == "C4sum":
+        P, logN, batch, n = presets.PRESETS["BGV_N15QP880"], 15, 128, 1 << 15
+        desc = "BGV N15QP880, batch 128 at level 19: InnerSum(1, N) = PartialTracesSum(1, N/2) + RotateRows + Add"
+    else:
+        P, logN, batch, n = presets.PRESETS["CKKS_PN16QP1761"], 16, 64, 7
+        desc = "CKKS PN16QP1761, batch 64 at level 33: RotateAndAdd(1, 7) = PartialTracesSum(1, 7) (2 doublings + 2 lazy QP terms)"
+    ctx = lb.Context(logN, P["Q"], P["P"])
+    N = ctx.N
+    level, levelP = len(P["Q"]) - 1, len(P["P"]) - 1
+    gal = lambda k: pow(5, k & (2 * N - 1), 2 * N)
+    pts_n = n // 2 if name == "C4sum" else n
+    els = set()
+    for lazy, dbl in _pts_schedule(ctx, 1, pts_n):
+        els.add(gal(dbl))
+        if lazy is not None:
+            els.add(gal(lazy))
+    if name == "C4sum":
+        els.add(2 * N - 1)
+    keys = {g: lb.GadgetCiphertext(ctx, rand_evk(ctx, level, levelP, rng, dev), level, levelP) for g in sorted(els)}
+    ev = lb.innersum.Evaluator(ctx, keys)
+    rl = lb.Evaluator(ctx)
+    ct = rand_rows(ctx.Q, N, batch * 2, rng, dev).view(batch, 2, level + 1, N)
+    out_f, out_c = torch.empty_like(ct), torch.empty_like(ct)
+    tmp = torch.empty_like(ct)
+
+    def fused():
+        if name == "C4sum":
+            ev.InnerSum(ct, 1, n, out_f, N, bgv=True)
+        else:                                     # InnerSum itself rejects n * batchSize = 7 (not a power of two)
+            ev.RotateAndAdd(ct, 1, n, out_f)
+
+    def composed():
+        composed_pts(ctx, rl, keys, ct, 1, pts_n, out_c)
+        if name == "C4sum":                       # RotateRows + Add
+            rl.Automorphism(out_c, 2 * N - 1, keys[2 * N - 1], tmp)
+            ctx.ringQ.Add(out_c.view(-1, level + 1, N), tmp.view(-1, level + 1, N), out_c.view(-1, level + 1, N))
+    res = {}
+    fused(); composed(); torch.cuda.synchronize()
+    same = bool(torch.equal(out_f, out_c))
+    Sl = lambda l: l * N * 8
+    alg = batch * 4 * Sl(level + 1) + len(keys) * rand_evk_digits(level, levelP) * 2 * Sl(level + 1 + levelP + 1)
+    for tag, fn in (("fused", fused), ("composed", composed)):
+        launches = lb.lib().lgpu_launch_count()
+        fn(); torch.cuda.synchronize()
+        launches = lb.lib().lgpu_launch_count() - launches
+        med, mn = timeit(fn, iters, 3, flush)
+        res["%s_%s" % (name, tag)] = {"workload": desc + (" (one call)" if tag == "fused" else " (composed from existing entry points)"),
+                                      "ms_per_batch": med * 1e3, "ct_per_s": batch / med, "alg_bytes_per_batch": alg, "alg_GBs": alg / med / 1e9,
+                                      "launches_per_call": int(launches), "key_switches": len(_pts_schedule(ctx, 1, pts_n)) +
+                                      sum(1 for lz, _ in _pts_schedule(ctx, 1, pts_n) if lz is not None) + (1 if name == "C4sum" else 0),
+                                      "outputs_equal_fused_vs_composed": same}
+    res["%s_fused" % name]["speedup_vs_composed"] = res["%s_composed" % name]["ms_per_batch"] / res["%s_fused" % name]["ms_per_batch"]
+    del keys, ev
+    ctx.close()
+    return res
+
+
+def rand_evk_digits(levelQ, levelP):
+    return (levelQ + levelP + 1) // (levelP + 1)
 
 
 def main():
@@ -171,6 +296,10 @@ def main():
                          "ms_per_batch": med * 1e3, "ct_per_s": batch / med, "alg_bytes_per_batch": alg, "alg_GBs": alg / med / 1e9}
             ev.close()
         ctx.close()
+
+    for name in ("C4sum", "C3sum"):
+        if on(name):
+            res.update(bench_innersum(name, args.iters, rng, dev, flush))
 
     if on("BOOT"):
         P = presets.PRESETS["BOOT_N16QP1767"]
