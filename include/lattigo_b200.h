@@ -319,6 +319,38 @@ int lgpu_evaluator_partial_traces_sum(lgpu_ctx* ctx, int level, const uint64_t* 
 int lgpu_evaluator_trace(lgpu_ctx* ctx, int level_in, const uint64_t* ct_in, int is_ntt, int log_n, const lgpu_galois_keys* gks,
                          uint64_t* ct_out, int level_out, int batch, void* stream);
 
+/* ---- ring packing (core/rlwe/ring_packing.go), Standard ring only -------------------------------------------------------------
+ * RingPackingEvaluator.Expand / Pack on a single ring degree (the evaluator's MinLogN == MaxLogN == ctx LogN; with MinLogN < MaxLogN
+ * the caller keeps Split / Merge and calls these at MinLogN). At every step of either tree all key switches use one Galois element:
+ * they go through one gadget product per step per batch_chunk() ciphertexts (key read once per sub-batch). Keys are whatever
+ * lgpu_gadget_product accepts (multiple P, single P, BaseTwoDecomposition, levelP < MaxLevelP); only the steps that key-switch look
+ * theirs up, all of them before any device work (the reference fails at the first missing key after part of the work). The argument
+ * checks also run on a host-only ctx. Results equal the reference bit for bit.
+ * Errors common to both: a ConjugateInvariant ctx (the reference's messages), a missing key ("GaloisKey[g] is missing") or one that
+ * lgpu_gadget_product rejects, overlapping input and output, misalignment. */
+/* RingPackingEvaluator.Expand (:457-571). ct_in: [batch][2][level+1][N], is_ntt its domain. ct_out: [batch][N >> log_gap][2][level+1][N];
+ * element k of a batch entry is the reference's cts[k << log_gap]. Outputs are ALWAYS in the NTT domain: for a coefficient-domain
+ * input the reference marks cts[0] as NTT after transforming it, so its trailing INTT loop (:563-569) never fires. 0 <= log_gap <=
+ * LogN ("Expand: logGap out of range [0, LogN]"; the reference does not check it). Keys: N / 2^i + 1 for 0 <= i < LogN
+ * (GaloisElementsForExpand(LogN)). Scratch: max(1, S / 2) * batch ciphertexts (S = N >> log_gap) + min(batch_chunk(), S / 2 * batch)
+ * key-switch outputs + the gadget product's own; ct_out itself also serves as a scratch block before the last step writes it. */
+int lgpu_ring_packing_expand(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int is_ntt, int log_gap,
+                             const lgpu_galois_keys* gks, uint64_t* ct_out, int batch, void* stream);
+/* RingPackingEvaluator.Pack (:600-770). cts_in: [batch][n_cts][2][level+1][N], all at one level, is_ntt their domain; idx: HOST array
+ * of the n_cts map keys, sorted (the reference sorts them; here every consecutive pair is checked, with getMinimumGap's messages
+ * "getMinimumGap: invalid index list: element must be sorted from smallest to largest" / "...: contains duplicated elements").
+ * Keys >= 2^input_log_gap (or < 0) take part in the gap only, as in the reference. ct_out: [batch][2][level+1][N], NTT domain.
+ * cts_in is NOT modified (the reference NTTs and rescales its inputs in place). 0 <= input_log_gap <= LogN
+ * ("Pack: inputLogGap out of range [0, LogN]"; unchecked in the reference). Errors: n_cts <= 0 ("len(cts) = 0"), logStart >= logEnd
+ * ("gaps between ciphertexts is smaller than inputLogGap > N"), and no input reaching slot 0 ("Pack: no input ciphertext reaches
+ * slot 0 ..."): the reference returns a nil ciphertext with a nil error there. Keys: NthRoot - 1 at tree level 0 (reached only with
+ * input_log_gap = LogN) and GaloisElement(2^(i-1)) at level i >= 1 (GaloisElementsForPack). Scratch: (pairs of the first step) *
+ * batch ciphertexts + 2 * min(batch_chunk(), that) for the key-switch input and output of one sub-batch (+ batch ciphertexts
+ * per index in [0, 2^input_log_gap) for a coefficient-domain input: the NTT of the inputs the tree reads) + the gadget product's own. */
+int lgpu_ring_packing_pack(lgpu_ctx* ctx, int level, const uint64_t* cts_in, int is_ntt, const int* idx, int n_cts,
+                           int input_log_gap, int zero_garbage_slots, const lgpu_galois_keys* gks, uint64_t* ct_out,
+                           int batch, void* stream);
+
 /* ---- RGSW (core/rgsw) --------------------------------------------------------------------------------------------------
  * rgsw.Evaluator.ExternalProduct (core/rgsw/evaluator.go:39-88): RLWE x RGSW -> RLWE at the RGSW ciphertext's levels.
  * rgsw0 / rgsw1 = rgsw.Ciphertext.Value[0] / Value[1] (core/rgsw/elements.go:11-13). ct_in: [batch][2][level_in+1][N], NTT domain;

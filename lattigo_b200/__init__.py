@@ -10,6 +10,7 @@ from .ringqp import RingQP, Poly as PolyQP  # noqa: F401
 from .bgv import BGVEvaluator  # noqa: F401
 from . import lintrans  # noqa: F401,E402
 from . import innersum  # noqa: F401,E402
+from . import ringpacking  # noqa: F401,E402
 from . import wire  # noqa: F401,E402
 from . import rgsw  # noqa: F401,E402
 from . import encryptor  # noqa: F401,E402

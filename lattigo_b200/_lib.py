@@ -87,6 +87,8 @@ def lib():
             "lgpu_evaluator_automorphism_hoisted_lazy": [vp, i, vp, vp, i, u64, vp, vp, vp, vp, vp, i, z, z, z, vp],
             "lgpu_evaluator_partial_traces_sum": [vp, i, vp, i, i, i, vp, vp, i, vp],
             "lgpu_evaluator_trace": [vp, i, vp, i, i, vp, vp, i, i, vp],
+            "lgpu_ring_packing_expand": [vp, i, vp, i, i, vp, vp, i, vp],
+            "lgpu_ring_packing_pack": [vp, i, vp, i, vp, i, i, i, vp, vp, i, vp],
             "lgpu_rgsw_external_product": [vp, vp, i, vp, vp, vp, i, i, vp],
             "lgpu_sample_uniform": [vp, i, i, u64, u64, vp, i, z, vp],
             "lgpu_sample_ternary": [vp, c.c_double, i, u64, u64, vp, i, vp],

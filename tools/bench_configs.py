@@ -19,6 +19,10 @@ produces the per-config table that DESIGN.md quotes and writes it as JSON (defau
   lgpu_evaluator_automorphism_hoisted_lazy, lgpu_evaluator_automorphism with the hoisted decomposition, vecops, ModDown) in the
   same run, and report the kernel launches of one call. Algorithmic bytes: every input and output ciphertext once plus every
   Galois key once.
+  C4expand  BGV N15QP880 at level 3, one ciphertext: RingPackingEvaluator.Expand(logGap = 7), 256 outputs (262 key switches)
+  C4pack    the 256 outputs of C4expand: Repack = Pack(cts, LogN, true) back into one ciphertext (262 key switches)
+  C4expand / C4pack also time the same schedule issued one ciphertext at a time from the existing entry points
+  (lgpu_evaluator_automorphism + vecops, what a shim looping like the reference does) and check that both give the same output.
 """
 import argparse
 import json
@@ -188,6 +192,137 @@ def bench_innersum(name, iters, rng, dev, flush):
     return res
 
 
+def _xpow2_ntt(ctx, level, div):
+    """GenXPow2NTT (core/rlwe/ring_packing.go:773-810) on the device: X^(+-2^i) in the NTT domain, Montgomery form."""
+    N, nq = ctx.N, level + 1
+    ringQ = ctx.ringQ.AtLevel(level)
+    x = torch.zeros((nq, N), dtype=torch.int64, device="cuda:0")
+    for i, q in enumerate(ctx.Q[:nq]):
+        x[i, N - 1 if div else 1] = int(((1 << 64) % q))
+    ringQ.NTT(x, x)
+    xs = [x]
+    for _ in range(1, ctx.logN):
+        y = torch.empty_like(x)
+        ringQ.MulCoeffsMontgomery(xs[-1], xs[-1], y)
+        xs.append(y)
+    if div:
+        ringQ.Neg(xs[0], xs[0])
+    return [t.expand(2, nq, N).contiguous() for t in xs]
+
+
+def _scale(ctx, level, x, s):
+    """x *= 2^-s mod Q_level (MulScalarBigint) on a (2, level+1, N) ciphertext."""
+    inv = [((pow(1 << s, -1, q)) << 64) % q for q in ctx.Q[: level + 1]]
+    ctx.ringQ.AtLevel(level).MulRNSScalarMontgomery(x, inv, x)
+
+
+def composed_expand(ctx, rl, keys, ct, logGap, xinv, out):
+    """Expand(ct, logGap) of one NTT-domain ciphertext, one Evaluator.Automorphism per ciphertext plus vecops (ring_packing.go:457-571).
+    out: (1, N >> logGap, 2, level+1, N); slot k holds cts[k << logGap]."""
+    level, N, gap = ct.shape[-2] - 1, ctx.N, 1 << logGap
+    ringQ = ctx.ringQ.AtLevel(level)
+    cts = {0: out[0, 0]}
+    cts[0].copy_(ct[0])
+    _scale(ctx, level, cts[0], ctx.logN)
+    tmp = torch.empty_like(cts[0])
+    for i in range(ctx.logN):
+        n = 1 << i
+        g = N // n + 1
+        for j in range(0, n, gap):
+            c0 = cts[j]
+            rl.Automorphism(c0, g, keys[g], tmp)
+            if n >= gap:
+                c1 = out[0, (j + n) // gap]
+                ringQ.Sub(c0, tmp, c1)
+                ringQ.Add(c0, tmp, c0)
+                ringQ.MulCoeffsMontgomery(c1, xinv[i], c1)
+                cts[j + n] = c1
+            else:
+                ringQ.Add(c0, tmp, c0)
+
+
+def composed_pack(ctx, rl, keys, cts_in, xpow, out):
+    """Repack(cts) = Pack(cts, LogN, true) of NTT-domain ciphertexts, one Evaluator.Automorphism per ciphertext plus vecops
+    (ring_packing.go:600-770); cts_in is left as it was."""
+    keys_sorted = sorted(cts_in)
+    level, logN = cts_in[keys_sorted[0]].shape[-2] - 1, ctx.logN
+    ringQ = ctx.ringQ.AtLevel(level)
+    cts = {k: v.clone() for k, v in cts_in.items()}
+    for v in cts.values():
+        _scale(ctx, level, v, logN)
+    tmpa = torch.empty_like(out)
+    for i in range(logN):
+        t = 1 << (logN - 1 - i)
+        g = 2 * ctx.N - 1 if i == 0 else pow(5, 1 << (i - 1), 2 * ctx.N)
+        for jx in range(t):
+            a, b = cts.get(jx), cts.get(jx + t)
+            if b is not None:
+                ringQ.MulCoeffsMontgomery(b, xpow[logN - i - 1], b)
+                if a is not None:
+                    ringQ.Sub(a, b, tmpa)
+                    ringQ.Add(a, b, a)
+                else:
+                    cts[jx] = b
+                cts[jx + t] = None
+            if a is not None:
+                rl.Automorphism(tmpa if b is not None else a, g, keys[g], tmpa)
+                ringQ.Add(a, tmpa, a)
+            elif b is not None:
+                rl.Automorphism(b, g, keys[g], tmpa)
+                ringQ.Sub(b, tmpa, b)
+    out.copy_(cts[0])
+
+
+def bench_ringpacking(iters, rng, dev, flush):
+    P, logN, level, logGap = presets.PRESETS["BGV_N15QP880"], 15, 3, 7
+    ctx = lb.Context(logN, P["Q"], P["P"])
+    N, levelP = ctx.N, len(P["P"]) - 1
+    els = sorted(set(lb.ringpacking.GaloisElementsForExpand(ctx, logN)) | set(lb.ringpacking.GaloisElementsForPack(ctx, logN)))
+    keys = {g: lb.GadgetCiphertext(ctx, rand_evk(ctx, level, levelP, rng, dev), level, levelP) for g in els}
+    ev = lb.ringpacking.RingPackingEvaluator(ctx, keys, keys)
+    rl = lb.Evaluator(ctx)
+    S = N >> logGap
+    ct = rand_rows(ctx.Q[: level + 1], N, 2, rng, dev).view(1, 2, level + 1, N)
+    xinv, xpow = _xpow2_ntt(ctx, level, True), _xpow2_ntt(ctx, level, False)
+    out_c = torch.empty((1, S, 2, level + 1, N), dtype=torch.int64, device=dev)
+    got = {}
+    packed_c = torch.empty((2, level + 1, N), dtype=torch.int64, device=dev)
+
+    def expand_f():
+        got["e"] = ev.Expand(ct, logGap)
+
+    def expand_c():
+        composed_expand(ctx, rl, keys, ct, logGap, xinv, out_c)
+    expand_f(); expand_c(); torch.cuda.synchronize()
+    cts = {k: v[0] for k, v in got["e"].items()}                     # (2, level+1, N) views of the device output
+
+    def pack_f():
+        got["p"] = ev.Repack(cts)
+
+    def pack_c():
+        composed_pack(ctx, rl, keys, cts, xpow, packed_c)
+    pack_f(); pack_c(); torch.cuda.synchronize()
+    same = {"C4expand": all(torch.equal(got["e"][k << logGap][0], out_c[0, k]) for k in range(S)), "C4pack": bool(torch.equal(got["p"], packed_c))}
+    Sl = lambda l: l * N * 8
+    key_bytes = rand_evk_digits(level, levelP) * 2 * Sl(level + 1 + levelP + 1)
+    res = {}
+    for name, f, c, desc in (("C4expand", expand_f, expand_c, "BGV N15QP880 at level 3, one ciphertext: Expand(logGap = 7) -> 256 ciphertexts"),
+                             ("C4pack", pack_f, pack_c, "BGV N15QP880 at level 3: Repack of the 256 Expand outputs into one ciphertext")):
+        for tag, fn in (("batched", f), ("per_ciphertext", c)):
+            launches = lb.lib().lgpu_launch_count()
+            fn(); torch.cuda.synchronize()
+            launches = lb.lib().lgpu_launch_count() - launches
+            med, mn = timeit(fn, iters, 2, flush)
+            res["%s_%s" % (name, tag)] = {"workload": desc + (" (one call, one gadget product per tree step)" if tag == "batched" else
+                                                              " (one Evaluator.Automorphism per ciphertext + vecops)"),
+                                          "ms_per_call": med * 1e3, "ms_min": mn * 1e3, "launches_per_call": int(launches), "key_switches": 262,
+                                          "galois_key_bytes": key_bytes, "outputs_equal_batched_vs_per_ciphertext": same[name]}
+        res["%s_batched" % name]["speedup_vs_per_ciphertext"] = res["%s_per_ciphertext" % name]["ms_per_call"] / res["%s_batched" % name]["ms_per_call"]
+    del keys, ev
+    ctx.close()
+    return res
+
+
 def rand_evk_digits(levelQ, levelP):
     return (levelQ + levelP + 1) // (levelP + 1)
 
@@ -300,6 +435,9 @@ def main():
     for name in ("C4sum", "C3sum"):
         if on(name):
             res.update(bench_innersum(name, args.iters, rng, dev, flush))
+
+    if on("C4expand") or on("C4pack"):
+        res.update(bench_ringpacking(args.iters, rng, dev, flush))
 
     if on("BOOT"):
         P = presets.PRESETS["BOOT_N16QP1767"]
