@@ -351,6 +351,27 @@ int lgpu_ring_packing_pack(lgpu_ctx* ctx, int level, const uint64_t* cts_in, int
                            int input_log_gap, int zero_garbage_slots, const lgpu_galois_keys* gks, uint64_t* ct_out,
                            int batch, void* stream);
 
+/* ---- generic key switch with ring-degree switching (core/rlwe/evaluator_evaluationkey.go, core/rlwe/element.go) --------------
+ * Evaluator.ApplyEvaluationKey (:36-107) for a batch of degree-1 ciphertexts sharing one evaluation key. ctx is the evaluator,
+ * i.e. the LARGE ring degree N. ct_in: [batch][2][level_in+1][2^log_n_in], ct_out: [batch][2][level_out+1][2^log_n_out], both in
+ * the domain is_ntt gives. Rows 0..min(level_in, level_out) of each component of ct_out are written; the block keeps its layout.
+ *   n_in == n_out == N   ct_out = (c0 + ks0, ks1), ks = GadgetProduct(c1); ct_out == ct_in is allowed (with level_out == level_in)
+ *   n_in <  n_out == N   SwitchCiphertextRingDegree[NTT] to X^(N/n_in) into ct_out, then the key switch in place. In the coefficient
+ *                        domain only every gap-th coefficient of ct_out is written by the map, as in the reference
+ *   n_in == N >  n_out   key switch at N, then SwitchCiphertextRingDegree[NTT] down to n_out (the NTT case as one block-average
+ *                        pass, DESIGN 3.4)
+ * Any other overlap of ct_in and ct_out is rejected. One gadget product runs per batch_chunk() ciphertexts (the key is read once per
+ * sub-batch). The evaluation key is whatever lgpu_gadget_product accepts at level min(level_in, level_out).
+ * Errors, all checked before any device work (also on a host-only ctx): "cannot ApplyEvaluationKey: opOut ring degree does not match
+ * evaluator params ring degree" and the ctIn variant (the reference's messages), equal degrees other than N, a degree below 2^4,
+ * a degree switch on a ConjugateInvariant ctx (the reference supports it; here only the same-degree case runs on that ring), a
+ * key level below min(level_in, level_out) (the reference adds rows the gadget product did not write there), and any key
+ * lgpu_gadget_product rejects. Where the reference panics because ct_out has more rows than ct_in (both directions in the
+ * coefficient domain, downward in the NTT domain), the rows above min(level_in, level_out) are left as they were. */
+int lgpu_evaluator_apply_evaluation_key(lgpu_ctx* ctx, const uint64_t* ct_in, int log_n_in, int level_in, int is_ntt,
+                                        const lgpu_gadget_ct* evk, uint64_t* ct_out, int log_n_out, int level_out,
+                                        int batch, void* stream);
+
 /* ---- RGSW (core/rgsw) --------------------------------------------------------------------------------------------------
  * rgsw.Evaluator.ExternalProduct (core/rgsw/evaluator.go:39-88): RLWE x RGSW -> RLWE at the RGSW ciphertext's levels.
  * rgsw0 / rgsw1 = rgsw.Ciphertext.Value[0] / Value[1] (core/rgsw/elements.go:11-13). ct_in: [batch][2][level_in+1][N], NTT domain;

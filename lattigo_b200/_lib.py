@@ -89,6 +89,7 @@ def lib():
             "lgpu_evaluator_trace": [vp, i, vp, i, i, vp, vp, i, i, vp],
             "lgpu_ring_packing_expand": [vp, i, vp, i, i, vp, vp, i, vp],
             "lgpu_ring_packing_pack": [vp, i, vp, i, vp, i, i, i, vp, vp, i, vp],
+            "lgpu_evaluator_apply_evaluation_key": [vp, vp, i, i, i, vp, vp, i, i, i, vp],
             "lgpu_rgsw_external_product": [vp, vp, i, vp, vp, vp, i, i, vp],
             "lgpu_sample_uniform": [vp, i, i, u64, u64, vp, i, z, vp],
             "lgpu_sample_ternary": [vp, c.c_double, i, u64, u64, vp, i, vp],

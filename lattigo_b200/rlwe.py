@@ -194,6 +194,23 @@ class Evaluator:
         level = ctIn.shape[-2] - 1
         _lib.check(_lib.lib().lgpu_evaluator_relinearize(self.ctx.h, level, _dptr(ctIn), rlk.ref(), _dptr(ctOut), b, _stream()))
 
+    def ApplyEvaluationKey(self, ctIn, evk: GadgetCiphertext, ctOut, is_ntt: bool = True):
+        """Evaluator.ApplyEvaluationKey (core/rlwe/evaluator_evaluationkey.go:36-107) on (2, level+1, n) or (batch, 2, level+1, n)
+        ciphertexts. The ring degrees are the tensors' last dimensions; this evaluator's context is the larger one. Rows
+        0..min(levels) of ctOut are written; ctOut may be ctIn at the same degree."""
+        b, _ = _bs(ctIn, 3)
+        bo, _ = _bs(ctOut, 3)
+        if b != bo:
+            raise ValueError("ApplyEvaluationKey: ctIn and ctOut batch sizes differ")
+        log_n = []
+        for t in (ctIn, ctOut):
+            n = t.shape[-1]
+            if n <= 0 or n & (n - 1):
+                raise ValueError("ApplyEvaluationKey: ring degree %d is not a power of two" % n)
+            log_n.append(n.bit_length() - 1)
+        _lib.check(_lib.lib().lgpu_evaluator_apply_evaluation_key(self.ctx.h, _dptr(ctIn), log_n[0], ctIn.shape[-2] - 1, 1 if is_ntt else 0, evk.ref(),
+                                                                  _dptr(ctOut), log_n[1], ctOut.shape[-2] - 1, b, _stream()))
+
 
 class CKKSEvaluator(Evaluator):
     """ckks.Evaluator: MulRelinNew (schemes/ckks/evaluator.go:719-872) and Rescale (:477-515) for degree-1

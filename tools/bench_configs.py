@@ -23,8 +23,13 @@ produces the per-config table that DESIGN.md quotes and writes it as JSON (defau
   C4pack    the 256 outputs of C4expand: Repack = Pack(cts, LogN, true) back into one ciphertext (262 key switches)
   C4expand / C4pack also time the same schedule issued one ciphertext at a time from the existing entry points
   (lgpu_evaluator_automorphism + vecops, what a shim looping like the reference does) and check that both give the same output.
+  C3aek_down / C3aek_up  CKKS PN16QP1761, batch 64 at level 33, NTT domain: Evaluator.ApplyEvaluationKey 2^16 -> 2^15 and
+         2^15 -> 2^16 through lgpu_evaluator_apply_evaluation_key, against the same work composed from the existing entry points
+         (GadgetProduct + Add + INTT at 2^16 + a strided copy + NTT at 2^15 going down; MapSmallDimensionToLargerDimensionNTT +
+         GadgetProduct + Add going up), with both outputs compared.
 """
 import argparse
+import ctypes
 import json
 import os
 import sys
@@ -323,6 +328,59 @@ def bench_ringpacking(iters, rng, dev, flush):
     return res
 
 
+def bench_apply_evk(iters, rng, dev, flush):
+    P = presets.PRESETS["CKKS_PN16QP1761"]
+    big, small = lb.Context(16, P["Q"], P["P"]), lb.Context(15, P["Q"], P["P"])
+    level, levelP, B = len(P["Q"]) - 1, len(P["P"]) - 1, 64
+    N, n, nq = big.N, small.N, level + 1
+    key = lb.GadgetCiphertext(big, rand_evk(big, level, levelP, rng, dev), level, levelP)
+    rl = lb.Evaluator(big)
+    ringL, ringS = big.ringQ.AtLevel(level), small.ringQ.AtLevel(level)
+    L = lb.lib()
+    res = {}
+    for name, n_in, n_out in (("C3aek_down", N, n), ("C3aek_up", n, N)):
+        # the composed arm keeps the two components apart, as a shim on rlwe.Ciphertext polynomials does
+        c0, c1 = rand_rows(big.Q, n_in, B, rng, dev), rand_rows(big.Q, n_in, B, rng, dev)
+        ct = torch.stack([c0, c1], dim=1).contiguous()
+        out_f = torch.empty((B, 2, nq, n_out), dtype=torch.int64, device=dev)
+        o0, o1 = (torch.empty((B, nq, n_out), dtype=torch.int64, device=dev) for _ in range(2))
+        ks0, ks1 = (torch.empty((B, nq, N), dtype=torch.int64, device=dev) for _ in range(2))
+        g = torch.empty((2, B, nq, N), dtype=torch.int64, device=dev)   # GadgetProduct's two outputs in one block: the fused ModDown applies
+
+        def fused():
+            rl.ApplyEvaluationKey(ct, key, out_f)
+        if n_out < n_in:
+            def composed():
+                rl.GadgetProduct(level, c1, key, g[0], g[1])
+                ringL.Add(c0, g[0], g[0])
+                ringL.INTT(g[0], g[0]); ringL.INTT(g[1], g[1])
+                ringS.NTT(g[0][..., ::2].contiguous(), o0); ringS.NTT(g[1][..., ::2].contiguous(), o1)
+        else:
+            def composed():
+                for src, dst in ((c0, ks0), (c1, ks1)):
+                    lb._lib.check(L.lgpu_map_small_dimension_to_larger_dimension_ntt(big.h, ctypes.c_void_p(src.data_ptr()), n, ctypes.c_void_p(dst.data_ptr()), N,
+                                                                                      B * nq, None))
+                rl.GadgetProduct(level, ks1, key, g[0], g[1])
+                ringL.Add(ks0, g[0], o0)                                  # component 1 is g[1]
+        fused(); composed(); torch.cuda.synchronize()
+        same = bool(torch.equal(out_f[:, 0], o0) and torch.equal(out_f[:, 1], o1 if n_out < n_in else g[1]))
+        row = {"workload": "CKKS PN16QP1761, batch %d at level %d, NTT domain: ApplyEvaluationKey 2^%d -> 2^%d" % (B, level, n_in.bit_length() - 1,
+                                                                                                                 n_out.bit_length() - 1),
+               "outputs_equal_fused_vs_composed": same}
+        for tag, fn in (("fused", fused), ("composed", composed)):
+            launches = L.lgpu_launch_count()
+            fn(); torch.cuda.synchronize()
+            launches = L.lgpu_launch_count() - launches
+            med, mn = timeit(fn, iters, 2, flush)
+            row[tag] = {"ms_per_batch": med * 1e3, "ms_min": mn * 1e3, "ct_per_s": B / med, "launches_per_call": int(launches)}
+        row["speedup_vs_composed"] = row["composed"]["ms_per_batch"] / row["fused"]["ms_per_batch"]
+        res[name] = row
+        del c0, c1, ct, out_f, o0, o1, ks0, ks1, g
+    del key
+    big.close(); small.close()
+    return res
+
+
 def rand_evk_digits(levelQ, levelP):
     return (levelQ + levelP + 1) // (levelP + 1)
 
@@ -438,6 +496,9 @@ def main():
 
     if on("C4expand") or on("C4pack"):
         res.update(bench_ringpacking(args.iters, rng, dev, flush))
+
+    if on("C3aek"):
+        res.update(bench_apply_evk(args.iters, rng, dev, flush))
 
     if on("BOOT"):
         P = presets.PRESETS["BOOT_N16QP1767"]
