@@ -290,6 +290,14 @@ struct LtState {
     const GaloisKeySet* gks;
 };
 
+// the key-level check of MultiplyByDiagMatrix[BSGS] (lintrans_evaluator.go:218-220, :410-412), with the reference's message
+static int check_key_level_p(int levelP, u64 galEl, const GadgetCt& gk) {
+    if (gk.levelP == levelP) return 0;
+    set_error("LinearTransformation.LevelP = " + std::to_string(levelP) + " != GaloiKey[" + std::to_string(galEl) + "].LevelP() = " +
+              std::to_string(gk.levelP) + ": ensure that the levelP of the linear transformation is the same as the levelP of the GaloisKeys");
+    return -1;
+}
+
 static const u64* diag_of(const LinTransView& m, int key) {
     for (int d = 0; d < m.n_diags; d++) if (m.diag_index[d] == key) return m.diag[d];
     return nullptr;
@@ -315,7 +323,7 @@ static int prerotate(const LtState& s, const std::vector<int>& rots, PreRot& pre
         const u64 galEl = galois_element(s.c, i);
         const GadgetCt* gk = s.gks->find(galEl);
         if (!gk) return -1;
-        if (gk->levelP != s.levelP) { set_error("LinearTransformation.LevelP != GaloisKey.LevelP()"); return -1; }
+        if (check_key_level_p(s.levelP, galEl, *gk)) return -1;
         std::unique_ptr<Buf> b(new Buf);
         b->st = s.st;
         LGPU_CUDA_OK(cudaMallocAsync((void**)&b->p, per * sizeof(u64), s.st));
@@ -354,7 +362,7 @@ static int multiply_naive(const LtState& s, const LinTransView& m, int levelQ, u
         const u64 galEl = galois_element(c, k);
         const GadgetCt* gk = s.gks->find(galEl);
         if (!gk) return -1;
-        if (gk->levelP != s.levelP) { set_error("LinearTransformation.LevelP != GaloisKey.LevelP()"); return -1; }
+        if (check_key_level_p(s.levelP, galEl, *gk)) return -1;
         // rotated hoisted product in one pass (the permutation is folded into it), then the diagonal multiply-accumulate without gather
         if (automorphism_hoisted_lazy(c, levelQ, CSpan{s.ctP, N, s.nqd * N}, s.decomp, s.levelQd, galEl, *gk, acc, s.batch, s.st)) return -1;
         const u64* pt = diag_of(m, keys[i]);
@@ -440,7 +448,7 @@ static int multiply_bsgs(const LtState& s, const LinTransView& m, const PreRot& 
             const u64 galEl = galois_element(c, j);
             const GadgetCt* gk = s.gks->find(galEl);
             if (!gk) return -1;
-            if (gk->levelP != s.levelP) { set_error("LinearTransformation.LevelP != GaloisKey.LevelP()"); return -1; }
+            if (check_key_level_p(s.levelP, galEl, *gk)) return -1;
             AccSpans g = stacked_acc(gb, nq, np, N, s.batch);
             if (gadget_product_lazy(c, levelQ, CSpan{t1d, N, nq * N}, *gk, g, s.batch, s.st)) return -1;
             if (launch_vecop(c, rqp, LGPU_OP_ADD, CSpan{gb, N, sbs}, CSpan{tb, N, sbs}, Span{gb, N, sbs}, s.batch, nullptr, nullptr, 0, 0, c->N, s.st)) return -1;

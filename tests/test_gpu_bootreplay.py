@@ -1,6 +1,7 @@
 """Smoke test of the bootstrapping op-trace replay (lattigo_b200/bootreplay.py, BASELINE config 5) on a reduced literal: every op kind of
 the trace runs through the C ABI at N = 2^13 and the per-phase timing covers the four phases. (The replay measures device time on
-synthetic operands; the arithmetic of each entry point is covered by its own parity test.)"""
+synthetic operands; the arithmetic of each entry point is covered by its own parity test. For the lintrans ops, that test runs the
+replay's own matrices and keys from this literal: tests/test_gpu_lintrans_shapes.py.)"""
 import pytest
 
 pytestmark = pytest.mark.gpu

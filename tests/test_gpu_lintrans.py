@@ -14,19 +14,41 @@ pytestmark = pytest.mark.gpu
 U64 = np.uint64
 
 
-def _setup(logN, lq, lp, mats, seed, batch=2, primes=None):
-    """mats: list of (rotations, N1, levelQ). Returns everything both sides need."""
+EDGE_POS = (0, 1, 2, 3, 5)       # coefficients set to 0, q - 1, q - 1, q - 1, 0 on every row by `edges=True`
+
+
+def _rand(moduli, N, rng, edges):
+    """Uniform residues; with `edges`, 0 and q - 1 at EDGE_POS of every row (the largest lazy sums of the MACs)."""
+    x = H.rand_poly(moduli, N, rng)
+    if edges:
+        top = np.array([int(m) - 1 for m in moduli], dtype=U64)
+        x[:, EDGE_POS[0]] = 0; x[:, EDGE_POS[4]] = 0
+        for c in EDGE_POS[1:4]:
+            x[:, c] = top
+    return x
+
+
+def _setup(logN, lq, lp, mats, seed, batch=2, primes=None, ring_type=0, log_slots=None, levelP=None, edges=False, ct_level=None):
+    """mats: list of (rotations, N1, levelQ). Returns everything both sides need.
+    ring_type: 0 standard, 1 conjugate invariant (primes = 1 mod 4N, NthRoot 4N). log_slots: the matrices' LogSlots
+    (default logN - 1 on the standard ring, logN on the conjugate-invariant one). levelP: the matrices' LevelP, at which the
+    Galois keys are made too (default the context's last P prime). primes: explicit (Q, P) lists. edges: 0 and q - 1 words at
+    EDGE_POS of the ciphertext, the diagonals and the keys. ct_level: level of the input ciphertexts (default the top)."""
     import lattigo_b200 as lb
     if primes is None:
-        q, p = O.gen_moduli(logN + 1, lq, lp)
+        q, p = O.gen_moduli(logN + 1 + ring_type, lq, lp)
     else:
         q, p = primes
-    params = O.Parameters(logN, q, p)
+    params = O.Parameters(logN, q, p, "ConjugateInvariant" if ring_type else "Standard")
     N = params.N()
     rng = np.random.default_rng(seed)
-    ctx = lb.Context(logN, q, p)
-    level, levelP = len(q) - 1, len(p) - 1
-    slots = N >> 1
+    ctx = lb.Context(logN, q, p, ring_type=ring_type)
+    level = len(q) - 1
+    levelP = len(p) - 1 if levelP is None else levelP
+    ct_level = level if ct_level is None else ct_level
+    if log_slots is None:
+        log_slots = logN if ring_type else logN - 1
+    slots = 1 << log_slots
     need = set()
     for rots, N1, _ in mats:
         if N1:
@@ -38,18 +60,23 @@ def _setup(logN, lq, lp, mats, seed, batch=2, primes=None):
     for r in sorted(need):
         g = params.GaloisElement(r)
         gk = H.random_gadget_ciphertext(params, level, levelP, rng)
+        if edges:
+            for d in range(gk.data.shape[0]):
+                for c in range(2):
+                    gk.data[d, 0, c] = _rand(q + p[: levelP + 1], N, rng, True)
         keys_o[g] = gk
         keys_d[g] = lb.GadgetCiphertext(ctx, gk.data, level, levelP)
     lts_o, lts_d = [], []
     for rots, N1, lvl in mats:
         vo, vd = {}, {}
         for r in rots:
-            dq = H.rand_poly(q[: lvl + 1], N, rng); dp = H.rand_poly(p, N, rng)
+            dq = _rand(q[: lvl + 1], N, rng, edges); dp = _rand(p[: levelP + 1], N, rng, edges)
             vo[r] = (dq, dp)
             vd[r] = ctx.to_device(np.concatenate([dq, dp]))
-        lts_o.append(LT.LinearTransformation(vo, lvl, levelP, logN - 1, N1))
-        lts_d.append(lb.lintrans.LinearTransformation(vd, lvl, levelP, logN - 1, N1))
-    ct = np.stack([np.stack([H.rand_poly(q, N, rng), H.rand_poly(q, N, rng)]) for _ in range(batch)])
+        lts_o.append(LT.LinearTransformation(vo, lvl, levelP, log_slots, N1))
+        lts_d.append(lb.lintrans.LinearTransformation(vd, lvl, levelP, log_slots, N1))
+    qc = q[: ct_level + 1]
+    ct = np.stack([np.stack([_rand(qc, N, rng, edges), _rand(qc, N, rng, edges)]) for _ in range(batch)])
     return lb, ctx, params, keys_o, keys_d, lts_o, lts_d, ct
 
 
