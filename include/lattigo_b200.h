@@ -185,7 +185,10 @@ int lgpu_modup_centered(lgpu_ctx* ctx, const uint64_t* row0, int first_q, int le
                         uint64_t* out_p, int batch, size_t stride_in, size_t stride_q, size_t stride_p, void* stream);
 
 /* ---- RNS basis extension (ring/basis_extension.go) -------------------------------------------------------
- * polQ has levelQ+1 rows, polP has levelP+1 rows; `batch` polynomials with the given strides (words). */
+ * polQ has levelQ+1 rows, polP has levelP+1 rows; `batch` polynomials with the given strides (words).
+ * One basis extension takes at most 64 source limbs (ModUpQtoP up to level_q = 63, ModUpPtoQ up to level_p = 63, and
+ * DecomposeAndSplit digits of up to 64 limbs); more returns an error. The reference's reconstructRNS stops at 32 source
+ * limbs; from 33 to 64 the result is its formula (same float64 `v`, same representative) applied to more limbs. */
 /* BasisExtender.ModUpQtoP (:177-190) / ModUpPtoQ (:195-209): outputs are the reference's exact (non-canonical,
  * < 2p) representatives. */
 int lgpu_modup_qtop(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t* pol_q, uint64_t* pol_p,

@@ -159,7 +159,8 @@ int lgpu_evaluator_moddown(lgpu_ctx* ctx, int lq, int lp, const uint64_t* a0q, c
 int lgpu_decompose_single_ntt(lgpu_ctx* ctx, int lq, int lp, int nb_pi, int digit, const uint64_t* c2ntt, const uint64_t* c2inv, uint64_t* c2q,
                               uint64_t* c2p, int batch, size_t si, size_t sq, size_t sp, void* stream) {
     REQUIRE_DEVICE(ctx);
-    REQUIRE(c2ntt && c2inv && c2q, "null polynomial");
+    REQUIRE(c2ntt && c2inv && c2q && (c2p || lp < 0), "null polynomial");
+    if (check_levels(ctx->c, lq, lp, lp >= 0)) return -1;
     const size_t N = ctx->c.N;
     return decompose_single_ntt(&ctx->c, lq, lp, nb_pi, digit, CSpan{(const u64*)c2ntt, N, si}, CSpan{(const u64*)c2inv, N, si}, Span{(u64*)c2q, N, sq},
                                 Span{(u64*)c2p, N, sp}, true, batch, S(stream));

@@ -616,6 +616,7 @@ def mod_up_exact(p1, p2, ringQ: Ring, ringP: Ring, muc: ModUpConstants):
     """ModUpExact, ring/basis_extension.go:282-308. p1: (levelQ+1, N), p2: (levelP+1, N)."""
     nQ, nP, n = p1.shape[0], p2.shape[0], p1.shape[1]
     assert p1.strides[1] == 8 and p2.strides[1] == 8
+    assert nQ <= 64, "lo_modup_exact holds at most 64 source limbs"
     Q = np.array(ringQ.ModuliChain()[:nQ], dtype=U64); mq = np.array([s.MRedConstant for s in ringQ.SubRings[:nQ]], dtype=U64)
     P = np.array(ringP.ModuliChain()[:nP], dtype=U64); mp = np.array([s.MRedConstant for s in ringP.SubRings[:nP]], dtype=U64)
     lib().lo_modup_exact(p1.ctypes.data, p1.strides[0] // 8, nQ, p2.ctypes.data, p2.strides[0] // 8, nP, n,
@@ -737,6 +738,7 @@ class Decomposer:
         QHalf = QBig >> 1
         nD = p0idxed - p0idxst
         assert nD == decompLvl + 2
+        assert nD <= 64, "lo_decompose_reconstruct holds at most 64 source limbs"
         Qd = np.array(Qc[p0idxst:p0idxed], dtype=U64)
         mq = np.array([ringQ.SubRings[i].MRedConstant for i in range(p0idxst, p0idxed)], dtype=U64)
         qh = np.array([QHalf % Qc[i] for i in range(p0idxst, p0idxed)], dtype=U64)

@@ -301,8 +301,9 @@ def test_edge_inputs_reach_the_float_v_edges():
 
 
 # ---- device runs ------------------------------------------------------------------------------------------------------------
-def _scopes(fn):
-    """Runs fn() with the event profiler on: (K2 scopes, epilogue scopes). The profiler keeps every chain on the caller's stream."""
+def _scopes(fn, classes=(7, 8)):
+    """Runs fn() with the event profiler on: (output, scopes of each of `classes`), by default LGPU_KCLASS_FUSED (K2) and
+    LGPU_KCLASS_EPILOGUE. The profiler keeps every chain on the caller's stream."""
     import torch
     lb = _lb()
     L = lb.lib()
@@ -318,7 +319,7 @@ def _scopes(fn):
     finally:
         L.lgpu_profile_enable(0)
     L.lgpu_profile_read(ms, by, sc, kn)
-    return out, int(sc[7]), int(sc[8])          # LGPU_KCLASS_FUSED, LGPU_KCLASS_EPILOGUE
+    return (out,) + tuple(int(sc[k]) for k in classes)
 
 
 def _check(ctx, got, want, what):
