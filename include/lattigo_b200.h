@@ -422,6 +422,21 @@ int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t
  * (GaloisElement(1..window_size) and NthRoot - GaloisGen; a missing one is an error). window_size = 10 in the reference (keys.go:14). */
 int lgpu_blind_rotate_core(lgpu_ctx* ctx, const uint64_t* a_host, int n_lwe, uint64_t* acc, int level, const lgpu_gadget_ct* brk0,
                            const lgpu_gadget_ct* brk1, const lgpu_galois_keys* gks, int window_size, void* stream);
+/* blindrot.Evaluator.Evaluate (core/rgsw/blindrot/evaluator.go:49-132) for a batch of LWE-ring ciphertexts: every listed slot of every
+ * ciphertext is blind-rotated in one call. ctx: the blind-rotation ring (N, Q); ctx_lwe: the LWE ring (N_LWE <= N, q_LWE; may be ctx).
+ * ct_lwe: [batch][2][level_lwe+1][N_LWE] in the domain is_ntt gives (the INTT runs in ctx_lwe); only level_lwe = 0 is supported (the
+ * reference switches higher levels to 2N with big integers). slots: HOST list of n_slots distinct indices in [0, N_LWE); test_polys[k]:
+ * the device rows (level+1 of them, stride N) of slot slots[k]'s test polynomial, NTT domain; slots may share a pointer. brk0[j] / brk1[j]
+ * (j < N_LWE <= n_brk): RGSW(X^{s_j}), all at the same levels and base; level = brk0[0].level_q. gks: the keys of GaloisElement(1..window_size)
+ * (except GaloisElement(v) = 1, which is a copy) and NthRoot - GaloisGen, all required before any device work. ct_out:
+ * [batch][n_slots][2][level+1][N], NTT domain, or coefficient domain when ntt_out = 0 (the reference's !NTTFlag branch).
+ * With level = 0, keys without P, BaseTwoDecomposition >= 1 and 2^8 <= N <= 2^12, every accumulator runs its whole Algorithm 3 in
+ * one CTA (csrc/blindrot.cu: at most three launches per call whatever batch, n_slots and N_LWE); otherwise each slot goes through
+ * lgpu_blind_rotate_core. Bit-identical to the reference in both cases. */
+int lgpu_blind_rotation_evaluate(lgpu_ctx* ctx, lgpu_ctx* ctx_lwe, const uint64_t* ct_lwe, int level_lwe, int is_ntt, const int* slots,
+                                 int n_slots, const uint64_t* const* test_polys, const lgpu_gadget_ct* brk0, const lgpu_gadget_ct* brk1,
+                                 int n_brk, const lgpu_galois_keys* gks, int window_size, int ntt_out, uint64_t* ct_out, int batch,
+                                 void* stream);
 /* ckks.SpecialFFTDouble / SpecialIFFTDouble (schemes/ckks/ckks_vector_ops.go:18-77; Encoder.FFT / IFFT, schemes/ckks/encoder.go:764-816), in
  * place on `batch` vectors of n complex128 values (device, interleaved re / im, batch_stride in complex values). rot_group (n int64 values)
  * and roots (m + 1 complex128 values) are the encoder's own tables (encoder.go:83-112), device resident. Same operations in the same order

@@ -99,6 +99,7 @@ def lib():
             "lgpu_encrypt_zero_sk": [vp, i, i, vp, vp, vp, vp, i, i, i, vp],
             "lgpu_gen_evaluation_key": [vp, vp, vp, vp, vp, vp],
             "lgpu_blind_rotate_core": [vp, vp, i, vp, i, vp, vp, vp, i, vp],
+            "lgpu_blind_rotation_evaluate": [vp, vp, vp, i, i, vp, i, vp, vp, vp, i, vp, i, i, vp, i, vp],
             "lgpu_ckks_special_fft": [vp, vp, i, i, vp, vp, i, i, z, vp],
             "lgpu_poly_load": [vp, vp, z, vp, i, vp, vp, vp],
             "lgpu_poly_store": [vp, vp, i, vp, z, vp, vp],

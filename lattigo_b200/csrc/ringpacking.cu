@@ -18,6 +18,7 @@
 #include "composite.h"
 #include "lintrans.h"
 #include "modarith.cuh"
+#include "xpow.cuh"
 
 namespace lgpu {
 
@@ -25,22 +26,6 @@ namespace lgpu {
 // kernels
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ u64 rp_sub(u64 a, u64 b, u64 q) { return a >= b ? a - b : a + q - b; }
-
-// slot j of NTT(X^k) is psi^(k * (2 brev(j) + 1)) (the evaluation order of the forward transform): psi^e = tw_fwd[brev(e)] for
-// e < N and -psi^(e - N) past it. x * that, canonical; k is taken mod 2N (k = 2N - n for X^-n).
-__device__ __forceinline__ u64 mul_xpow(u64 x, u64 k, u64 slot_odd, const LimbConst& L, int lg, u64 mask2n) {
-    u64 e = (k * slot_odd) & mask2n;
-    const u64 n = (mask2n + 1) >> 1, q = L.q;
-    const bool neg = e >= n;
-    if (neg) e -= n;
-    const ulonglong2 w = L.tw_fwd[__brevll(e) >> (64 - lg)];
-    const u64 r = cred(x * w.x - __umul64hi(x, w.y) * q, q);
-    return neg ? (r ? q - r : 0) : r;
-}
-__device__ __forceinline__ size_t auto_index(int j, u64 galEl, u64 mask2n, int lg) {     // ring/automorphism.go:12-34
-    const u64 tmp1 = 2 * (__brevll((u64)j) >> (64 - lg)) + 1;
-    return (size_t)(__brevll(((galEl * tmp1 & mask2n) - 1) >> 1) >> (64 - lg));
-}
 
 // one tree step of Pack: the pairs (jx, jy) that hold at least one ciphertext
 enum { PAIR_AB = 0, PAIR_A = 1, PAIR_B = 2 };

@@ -54,3 +54,26 @@ class BlindRotationEvaluator:
         assert len(a) == len(self.brk)
         _lib.check(_lib.lib().lgpu_blind_rotate_core(self.ctx.h, a.ctypes.data, len(a), _dptr(acc), acc.shape[-2] - 1, self._b0, self._b1,
                                                      ctypes.byref(self._gks), self.window, _stream()))
+
+    def Evaluate(self, ct_lwe, test_polys, ctx_lwe: Context = None, is_ntt: bool = True, ntt_out: bool = True):
+        """blindrot.Evaluator.Evaluate (core/rgsw/blindrot/evaluator.go:49-132) in one device call: ct_lwe is a level-0 LWE-ring ciphertext
+        (2, 1, N_LWE) or a batch (batch, 2, 1, N_LWE) in ctx_lwe (default: this evaluator's ring), in the NTT domain when is_ntt;
+        test_polys maps slot -> NTT-domain test polynomial (level+1, N). Returns {slot: (2, level+1, N) or (batch, 2, level+1, N)},
+        in the NTT domain unless ntt_out is False (the reference's !NTTFlag branch)."""
+        import ctypes
+        import torch
+        ctx_lwe = self.ctx if ctx_lwe is None else ctx_lwe
+        single = ct_lwe.dim() == 3
+        ct = ct_lwe.unsqueeze(0) if single else ct_lwe
+        ct = ct.contiguous()
+        slots = sorted(test_polys)
+        polys = [test_polys[s].contiguous() for s in slots]
+        level = self.brk[0].LevelQ()
+        N = self.ctx.N
+        out = torch.empty((ct.shape[0], len(slots), 2, level + 1, N), dtype=ct.dtype, device=ct.device)
+        c_slots = (ctypes.c_int * len(slots))(*slots)
+        c_polys = (ctypes.c_void_p * len(slots))(*[_dptr(p) for p in polys])
+        _lib.check(_lib.lib().lgpu_blind_rotation_evaluate(self.ctx.h, ctx_lwe.h, _dptr(ct), ct.shape[-2] - 1, int(is_ntt), c_slots, len(slots),
+                                                           c_polys, self._b0, self._b1, len(self.brk), ctypes.byref(self._gks), self.window,
+                                                           int(ntt_out), _dptr(out), ct.shape[0], _stream()))
+        return {s: (out[0, k] if single else out[:, k]) for k, s in enumerate(slots)}
