@@ -385,19 +385,29 @@ int lgpu_rgsw_external_product(lgpu_ctx* ctx, const uint64_t* ct_in, int level_i
 
 /* ---- encryptor / key-generator inner loops and device samplers (core/rlwe/encryptor.go, keygenerator.go, ring/sampler_*.go) ----
  * Samplers: the reference's distributions on Philox4x32-10 counter streams keyed by (seed, stream_id) -- NOT the reference's
- * blake2b-XOF byte stream (sampling/prng.go), which is inherently sequential. Small polynomials are int64 vectors [batch][N]. */
+ * blake2b-XOF byte stream (sampling/prng.go), which is inherently sequential. Small polynomials are int64 vectors [batch][N].
+ * Every block is philox4x32_10(counter, key) with key = (seed mod 2^32, (seed >> 32) ^ (stream_id >> 32) * 0x85EBCA6B mod 2^32)
+ * and counter = (c, poly | kind << 30, stream_id mod 2^32, attempt), kind = 0 uniform, 1 ternary {P}, 2 ternary {H}, 3 Gaussian:
+ *   uniform      c = coefficient, poly = batch index * 128 + global limb index (P limbs are nQ + j), one block per attempt;
+ *   ternary {P}  c = coefficient, poly = batch index, attempt = 0;
+ *   ternary {H}  c = attempt, poly = batch index, last word 0;
+ *   Gaussian     c = coefficient, poly = batch index, one block per attempt.
+ * Draws of different kinds therefore never share a block, and neither do the Q and P rows of one ringqp.Poly. Two calls of the
+ * same kind on the same (seed, stream_id) do: give every call its own stream_id (lattigo_b200.encryptor.Samplers does). This
+ * layout replaced one without the kind field, so output for a given (seed, stream_id) differs from builds before it. */
 /* ringqp.UniformSampler.Read (ring/sampler_uniform.go:48-100): rows 0..level uniform in [0, q_i). */
 int lgpu_sample_uniform(lgpu_ctx* ctx, int ring, int level, uint64_t seed, uint64_t stream_id, uint64_t* out, int batch,
                         size_t batch_stride, void* stream);
-/* ring.TernarySampler (ring/sampler_ternary.go): hamming_weight > 0 selects ring.Ternary{H} (exactly H non-zero coefficients),
- * otherwise ring.Ternary{P = p} (P(+1) = P(-1) = p / 2). */
+/* ring.TernarySampler (ring/sampler_ternary.go): hamming_weight > 0 selects ring.Ternary{H} (exactly min(H, N) non-zero
+ * coefficients), otherwise ring.Ternary{P = p} (P(+1) = P(-1) = ceil(p 2^53) / 2^54), p in (0, 1]. */
 int lgpu_sample_ternary(lgpu_ctx* ctx, double p, int hamming_weight, uint64_t seed, uint64_t stream_id, int64_t* out, int batch,
                         void* stream);
 /* ring.GaussianSampler (ring/sampler_gaussian.go:160-182): round(|N(0,1)| sigma) with a random sign, |.| <= bound. */
 int lgpu_sample_gaussian(lgpu_ctx* ctx, double sigma, double bound, uint64_t seed, uint64_t stream_id, int64_t* out, int batch,
                          void* stream);
 /* What Sampler.Read + ringqp.Ring.ExtendBasisSmallNormAndCenter (ring/ringqp/operations.go:325-351) leave in a ringqp.Poly:
- * the signed value modulo every q_i (out_q, level_q+1 rows) and p_j (out_p, level_p+1 rows); either output may be NULL. */
+ * the signed value modulo every q_i (out_q, level_q+1 rows) and p_j (out_p, level_p+1 rows); either output may be NULL.
+ * Precondition: |v| < q_0 / 2, where the reference's centring is exact (and |v| below every modulus written). */
 int lgpu_small_poly_to_rns(lgpu_ctx* ctx, int level_q, int level_p, const int64_t* small, uint64_t* out_q, uint64_t* out_p,
                            int batch, size_t stride_q, size_t stride_p, void* stream);
 /* Encryptor.encryptZeroPk for a plain rlwe.Ciphertext (core/rlwe/encryptor.go:204-299: one special prime, ModDownQPtoQ) or, when

@@ -9,8 +9,8 @@
 //   ringqp.Ring.ExtendBasisSmallNormAndCenter             ring/ringqp/operations.go:325-351 (folded into small_to_rns)
 // Samplers (ring/sampler_uniform.go, sampler_ternary.go, sampler_gaussian.go): same DISTRIBUTIONS, own random streams -- the
 // reference reads a blake2b XOF sequentially (sampling/prng.go), which has no parallel form; here every coefficient owns a
-// Philox4x32-10 counter (seed, stream, polynomial, coefficient, attempt), so a batch of polynomials is sampled in one launch and
-// the result does not depend on the launch geometry.
+// Philox4x32-10 counter (sampler kind, seed, stream, polynomial, coefficient, attempt), so a batch of polynomials is sampled in
+// one launch and the result does not depend on the launch geometry. The layout is restated bit for bit in oracle/philox.py.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -36,11 +36,18 @@ __device__ __forceinline__ Ph4 philox4x32_10(Ph4 c, unsigned k0, unsigned k1) {
     return c;
 }
 struct SampleKey { unsigned k0, k1, stream; };
-__device__ __forceinline__ Ph4 draw(const SampleKey& k, unsigned poly, unsigned coeff, unsigned attempt) {
-    return philox4x32_10(Ph4{coeff, poly, k.stream, attempt}, k.k0, k.k1);
+// Which sampler drew a block: bits 30..31 of the counter's polynomial word. The polynomial index itself stays below 2^23, so two
+// samplers of different kinds never share a Philox input, whatever the seed and stream id.
+enum SampleKind : unsigned { kKindUniform = 0, kKindTernaryP = 1, kKindTernaryH = 2, kKindGaussian = 3 };
+constexpr unsigned kKindShift = 30;
+static_assert(65535ull * kMaxRows + kMaxRows <= (1ull << kKindShift), "the polynomial index reaches the sampler-kind field");
+// counter words: (coefficient, polynomial | kind << 30, stream_id mod 2^32, attempt); key: make_key(seed, stream_id)
+__device__ __forceinline__ Ph4 draw(const SampleKey& k, SampleKind kind, unsigned poly, unsigned coeff, unsigned attempt) {
+    return philox4x32_10(Ph4{coeff, poly | (unsigned)kind << kKindShift, k.stream, attempt}, k.k0, k.k1);
 }
 
-// uniform in [0, q) per row: masked 64-bit words, rejected until below q (ring/sampler_uniform.go:48-100)
+// uniform in [0, q) per row: masked 64-bit words, rejected until below q (ring/sampler_uniform.go:48-100). The polynomial index is
+// batch * kMaxRows + global limb index (P limbs are nQ + j), so the Q and P rows of one ringqp.Poly drawn on one stream id differ.
 struct UniformParams {
     const LimbConst* limbs; RowMap rm;
     u64* out; size_t rs, bs;
@@ -52,10 +59,10 @@ __global__ void __launch_bounds__(256) sample_uniform_kernel(UniformParams p) {
     const int r = blockIdx.y, b = blockIdx.z;
     const u64 q = p.limbs[p.rm.limb[r]].q;
     const u64 mask = ~0ull >> __clzll((long long)(q - 1));
-    const unsigned poly = (unsigned)b * kMaxRows + (unsigned)r;
+    const unsigned poly = (unsigned)b * kMaxRows + (unsigned)p.rm.limb[r];
     u64 v = 0;
     for (unsigned a = 0;; a++) {
-        const Ph4 d = draw(p.key, poly, (unsigned)i, a);
+        const Ph4 d = draw(p.key, kKindUniform, poly, (unsigned)i, a);
         v = (((u64)d.x << 32) | d.y) & mask;
         if (v < q) break;
         v = (((u64)d.z << 32) | d.w) & mask;
@@ -64,16 +71,18 @@ __global__ void __launch_bounds__(256) sample_uniform_kernel(UniformParams p) {
     p.out[(size_t)b * p.bs + (size_t)p.rm.drow[r] * p.rs + i] = v;
 }
 
-// ternary with P(+-1) = prob / 2 each (ring.Ternary{P}, ring/sampler_ternary.go:136-201)
+// ternary with P(+-1) = prob / 2 each (ring.Ternary{P}, ring/sampler_ternary.go:136-201). u takes 53 bits, so it is exact and
+// below 1: P(non-zero) = ceil(prob * 2^53) / 2^53, and prob = 1 leaves no zero.
 __global__ void __launch_bounds__(256) sample_ternary_p_kernel(long long* out, int n, double prob, SampleKey key) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const Ph4 d = draw(key, blockIdx.y, (unsigned)i, 0);
-    const double u = ((double)d.x * 4294967296.0 + (double)d.y) * (1.0 / 18446744073709551616.0);
+    const Ph4 d = draw(key, kKindTernaryP, blockIdx.y, (unsigned)i, 0);
+    const double u = (double)(((u64)d.x << 21) | (d.y >> 11)) * (1.0 / 9007199254740992.0);   // [0, 1)
     out[(size_t)blockIdx.y * n + i] = u < prob ? ((d.z & 1u) ? 1 : -1) : 0;
 }
 // ternary with exactly h non-zero coefficients, uniform positions and signs (ring.Ternary{H}, :203-260): one CTA per polynomial,
-// positions drawn by rejection against a bitmap in shared memory
+// positions drawn by rejection against a bitmap in shared memory. Block a gives the candidates (d.x, sign d.y) then (d.z, sign d.w);
+// the polynomial's coefficients are the first h distinct positions of that sequence.
 __global__ void __launch_bounds__(256) sample_ternary_h_kernel(long long* out, int n, int h, SampleKey key) {
     extern __shared__ unsigned bitmap[];
     long long* o = out + (size_t)blockIdx.x * n;
@@ -83,7 +92,7 @@ __global__ void __launch_bounds__(256) sample_ternary_h_kernel(long long* out, i
     if (threadIdx.x != 0) return;
     int placed = 0;
     for (unsigned a = 0; placed < h; a++) {
-        const Ph4 d = draw(key, blockIdx.x, a, 0);
+        const Ph4 d = draw(key, kKindTernaryH, blockIdx.x, a, 0);
         const unsigned cand[2] = {d.x & (unsigned)(n - 1), d.z & (unsigned)(n - 1)};
         const unsigned sgn[2] = {d.y & 1u, d.w & 1u};
         for (int t = 0; t < 2 && placed < h; t++) {
@@ -102,7 +111,7 @@ __global__ void __launch_bounds__(256) sample_gaussian_kernel(long long* out, in
     if (i >= n) return;
     long long v = 0;
     for (unsigned a = 0;; a++) {
-        const Ph4 d = draw(key, blockIdx.y, (unsigned)i, a);
+        const Ph4 d = draw(key, kKindGaussian, blockIdx.y, (unsigned)i, a);
         const double u1 = ((double)(((u64)d.x << 21) | (d.y >> 11)) + 1.0) * (1.0 / 9007199254740992.0);   // (0, 1]
         const double u2 = (double)(((u64)d.z << 21) | (d.w >> 11)) * (1.0 / 9007199254740992.0);            // [0, 1)
         const double z = sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
@@ -117,7 +126,7 @@ __global__ void __launch_bounds__(256) sample_gaussian_kernel(long long* out, in
 }
 
 // signed small coefficients -> residues on the launch rows: Sampler.Read on the Q rows followed by ExtendBasisSmallNormAndCenter on
-// the P rows leaves exactly v mod q_i / v mod p_j (|v| < q_0 / 2)
+// the P rows leaves exactly v mod q_i / v mod p_j (|v| < q_0 / 2); the kernel's v mod q is exact for |v| < q
 struct SmallParams {
     const LimbConst* limbs; RowMap rm;
     const long long* in; size_t in_bs;
@@ -310,7 +319,7 @@ int lgpu_sample_ternary(lgpu_ctx* ctx, double p, int hamming_weight, uint64_t se
     const int N = ctx->c.N;
     count_launch(1);
     if (hamming_weight > 0) {
-        REQUIRE(hamming_weight <= N, "ternary sampler: Hamming weight above N");
+        if (hamming_weight > N) hamming_weight = N;      // as the reference does (ring/sampler_ternary.go:202-204)
         const size_t smem = (size_t)((N + 31) / 32) * sizeof(unsigned);
         sample_ternary_h_kernel<<<batch, 256, smem, (cudaStream_t)stream>>>((long long*)out, N, hamming_weight, make_key(seed, stream_id));
     } else {

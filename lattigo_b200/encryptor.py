@@ -11,7 +11,8 @@ from .rlwe import GadgetCiphertext
 
 
 class Samplers:
-    """Device samplers: the reference's distributions on counter-based streams keyed by (seed, stream id)."""
+    """Device samplers: the reference's distributions on counter-based streams keyed by (seed, stream id). Every call takes
+    one stream id, stream_id if given and otherwise the next of 1, 2, 3, ...; UniformQP draws both rings on that id."""
 
     def __init__(self, ctx: Context, seed: int):
         self.ctx, self.seed = ctx, seed & 0xFFFFFFFFFFFFFFFF
@@ -30,20 +31,18 @@ class Samplers:
 
     def UniformQP(self, levelQ: int, levelP: int, batch: int = 1, stream_id=None):
         """A uniform ringqp.Poly block (batch, levelQ+1 + levelP+1, N)."""
-        import torch
         sid = self._sid(stream_id)
         rows = levelQ + 1 + levelP + 1
-        out = torch.empty((batch, rows, self.ctx.N), dtype=torch.int64, device="cuda:%d" % self.ctx.device)
+        out = self.ctx.new_poly(rows, batch)
         L = _lib.lib()
-        _lib.check(L.lgpu_sample_uniform(self.ctx.h, RING_Q, levelQ, self.seed, 2 * sid, ctypes.c_void_p(out.data_ptr()), batch, rows * self.ctx.N, _stream()))
-        if levelP >= 0:
-            _lib.check(L.lgpu_sample_uniform(self.ctx.h, RING_P, levelP, self.seed, 2 * sid + 1,
+        _lib.check(L.lgpu_sample_uniform(self.ctx.h, RING_Q, levelQ, self.seed, sid, ctypes.c_void_p(out.data_ptr()), batch, rows * self.ctx.N, _stream()))
+        if levelP >= 0:      # the P limbs' counters differ from the Q limbs' (include/lattigo_b200.h), so the id is shared
+            _lib.check(L.lgpu_sample_uniform(self.ctx.h, RING_P, levelP, self.seed, sid,
                                              ctypes.c_void_p(out.data_ptr() + 8 * (levelQ + 1) * self.ctx.N), batch, rows * self.ctx.N, _stream()))
         return out
 
     def _small(self, batch):
-        import torch
-        return torch.empty((batch, self.ctx.N), dtype=torch.int64, device="cuda:%d" % self.ctx.device)
+        return self.ctx.new_poly(batch)
 
     def Ternary(self, P: float = 0.0, H: int = 0, batch: int = 1, stream_id=None):
         out = self._small(batch)

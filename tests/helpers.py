@@ -3,6 +3,7 @@ test infrastructure only)."""
 import numpy as np
 
 from oracle import oracle as O
+from oracle import philox as PH
 
 U64 = np.uint64
 
@@ -37,6 +38,54 @@ def launch_delta(fn):
     n0 = lb.lib().lgpu_launch_count()
     fn()
     return lb.lib().lgpu_launch_count() - n0
+
+
+def ntt_prime(bits, N, above):
+    """The NTT-friendly prime (1 mod 2N) closest to 2^bits from above or below."""
+    step = 2 * N
+    k = (1 << bits) // step + (1 if above else 0)
+    while not O.is_prime(k * step + 1):
+        k += 1 if above else -1
+    return k * step + 1
+
+
+def gof_pvalue(counts, probs, statistic="log-likelihood", min_expected=5.0):
+    """p-value of a G-test (or another scipy power-divergence statistic, e.g. "pearson") of observed counts against exact bin
+    probabilities; 0 if a bin of probability 0 has a draw. Bins are taken in order and merged until each expects at least
+    min_expected draws (a short last group joins the one before it)."""
+    from scipy.stats import power_divergence
+    counts = np.asarray(counts, dtype=np.float64)
+    probs = np.asarray(probs, dtype=np.float64)
+    if (counts[probs == 0] > 0).any():
+        return 0.0
+    o, e, acc_o, acc_e = [], [], 0.0, 0.0
+    for ci, ei in zip(counts, probs * counts.sum()):
+        acc_o += ci; acc_e += ei
+        if acc_e >= min_expected:
+            o.append(acc_o); e.append(acc_e); acc_o = acc_e = 0.0
+    if o:
+        o[-1] += acc_o; e[-1] += acc_e
+    if len(o) < 2:
+        return 1.0
+    return float(power_divergence(np.array(o), np.array(e) * (sum(o) / sum(e)), lambda_=statistic).pvalue)
+
+
+def uniform_pvalues(v, q):
+    """Chi-square p-values of uniform values in [0, q) over 256 equal bins and over the residue mod 3 (exact bin edges)."""
+    v = np.asarray(v, dtype=np.uint64)
+    edge = np.array([-(-k * q // 256) for k in range(257)], dtype=np.uint64)
+    bins = np.searchsorted(edge, v, side="right") - 1
+    p_bins = gof_pvalue(np.bincount(bins, minlength=256), PH.uniform_bin_probabilities(q, 256), "pearson")
+    p_res = gof_pvalue(np.bincount((v % np.uint64(3)).astype(np.int64), minlength=3), PH.uniform_residue_probabilities(q, 3), "pearson")
+    return p_bins, p_res
+
+
+def gaussian_edges(bound):
+    """Bin edges of |v| for oracle.philox.gaussian_law: one bin per value up to 64, else 80 bins of equal width."""
+    K = int(np.floor(bound + 0.5))
+    if K <= 64:
+        return list(range(K + 2))
+    return [0, 1] + [int(x) for x in np.unique(np.round(np.linspace(2, K + 1, 80)))]
 
 
 def small_poly_rns(coeffs, moduli):
