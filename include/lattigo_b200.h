@@ -487,6 +487,52 @@ int lgpu_ckks_mulrelin_rescale_batch(lgpu_ctx* ctx, int level, const uint64_t* c
 int lgpu_ckks_mulrelin_rescale_batch_host(lgpu_ctx* ctx, int level, const uint64_t* ct_a_host, const uint64_t* ct_b_host,
                                           const lgpu_gadget_ct* rlk, int nb_rescales, uint64_t* ct_out_host, int batch, int chunk);
 
+/* ---- CKKS polynomial evaluation (circuits/ckks/polynomial.Evaluator.Evaluate) ---------------------------------------
+ * A program planned on the host (lattigo_b200/polyeval.py restates the reference's power basis, Paterson-Stockmeyer split and
+ * scale bookkeeping) and run on a batch. Slots are single-assignment ciphertexts: slot 0 is the input (degree 1, `level`), every
+ * op writes one new slot (LINCOMB: n_out new slots) from slots written before it. The ops, one per rounding boundary:
+ *   MULRELIN dst = MulRelinNew(src0, src1)                 degree 1 x 1 -> 1, level = min(levels)
+ *   TENSOR   dst = r_b (src0 (x) src1) + r_a addend         degree 2; addend of degree 1 or 2 (-1: none, r_a unused);
+ *                                                           weights [2][level+1] = r_b, r_a per limb
+ *   RELIN    dst = Relinearize(src0)                        degree 2 -> 1
+ *   RESCALE  dst = Rescale(src0)                            levels_per_rescale x DivRoundByLastModulusNTT, degree kept
+ *   LINCOMB  outs[i] = sum_k W[i][k] terms[k] + W[i][n_terms] on component 0, rows 0..out_levels[i], per limb and NTT half
+ *            (slots < N/2 use half 0); weights [n_out][n_terms+1][level+1][2], level = max(out_levels); terms are degree 1,
+ *            and an output's weights of a term are 0 on rows above the term's level; n_terms <= LGPU_POLY_MAX_TERMS, n_out <= LGPU_POLY_MAX_OUTPUTS.
+ * `level` of every op is the level of what it writes; every weight is a canonical residue (< q_i). */
+#define LGPU_POLY_MULRELIN 0
+#define LGPU_POLY_TENSOR 1
+#define LGPU_POLY_RELIN 2
+#define LGPU_POLY_RESCALE 3
+#define LGPU_POLY_LINCOMB 4
+#define LGPU_POLY_MAX_TERMS 16
+#define LGPU_POLY_MAX_OUTPUTS 64
+typedef struct {
+    int kind;
+    int dst, src0, src1, addend;
+    int level;
+    int n_out, n_terms;
+    const int* outs;
+    const int* out_levels;
+    const int* terms;
+    const uint64_t* weights;   /* HOST */
+} lgpu_poly_op;
+typedef struct {
+    int n_slots;
+    int n_ops;
+    const lgpu_poly_op* ops;   /* HOST */
+    int out_slot;              /* degree 1, written by the last op */
+    int levels_per_rescale;
+} lgpu_poly_program;
+/* Runs `prog` on ct_in [batch][2][level+1][N] (NTT domain) into ct_out [batch][2][level_out+1][N], level_out the level of
+ * prog->out_slot. Equal bit for bit to the reference's op sequence when prog is what the planner emits for it. The whole program
+ * is checked before any launch, also on a host-only context: slot indices and single assignment, degrees and level arithmetic,
+ * term / output counts, every weight below its modulus, the relinearization key at every level it is used. Scratch: the slots are
+ * allocated when written and freed after their last read, per sub-batch of batch_chunk() ciphertexts; per ciphertext the peak is
+ * at most sum over slots of (degree+1)(level+1) N words plus the key-switch scratch of one MulRelinNew at `level`. */
+int lgpu_ckks_polynomial_evaluate(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                  const lgpu_gadget_ct* rlk, uint64_t* ct_out, void* stream);
+
 /* ---- BGV / BFV ciphertext multiplication (schemes/bgv) ---------------------------------------------------------
  * State of bgv.NewParameters' ringQMul + newEvaluatorPrecomp (schemes/bgv/params.go:98-109, evaluator.go:38-70) for the
  * context's Q: the plaintext modulus t, tMontgomery, levelQMul[] and the Q <-> QMul basis extender.

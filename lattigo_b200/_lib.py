@@ -80,6 +80,7 @@ def lib():
             "lgpu_evaluator_relinearize": [vp, i, vp, vp, vp, i, vp],
             "lgpu_ckks_mulrelin_rescale_batch": [vp, i, vp, vp, vp, i, vp, i, vp],
             "lgpu_ckks_mulrelin_rescale_batch_host": [vp, i, vp, vp, vp, i, vp, i, i],
+            "lgpu_ckks_polynomial_evaluate": [vp, i, vp, i, vp, vp, vp, vp],
             "lgpu_bgv_create": [vp, u64, vp, i, c.POINTER(vp)],
             "lgpu_bgv_destroy": [vp],
             "lgpu_bgv_mulrelin_batch": [vp, i, vp, vp, vp, i, i, vp, i, vp],
