@@ -453,6 +453,33 @@ int lgpu_blind_rotation_evaluate(lgpu_ctx* ctx, lgpu_ctx* ctx_lwe, const uint64_
  * as the Go code and no fused multiply-add: results are bit-identical on identical tables. */
 int lgpu_ckks_special_fft(lgpu_ctx* ctx, double* values, int n, int m, const int64_t* rot_group, const double* roots, int inverse,
                           int batch, size_t batch_stride, void* stream);
+/* ckks.Encoder on the prec <= 53 path, ring.Standard only (csrc/encoder.cu), bit-identical to the reference on identical rot_group / roots.
+ * flags: LGPU_ENC_NTT = MetaData.IsNTT, LGPU_ENC_MONTGOMERY = MetaData.IsMontgomery (encode; ignored by the non-batched Encode and by
+ * Decode, as in the reference), LGPU_ENC_COEFFS = IsBatched false. scale = MetaData.Scale.Float64(), finite and > 0. Strides are in
+ * elements (complex128 values, float64 values, or uint64 words); batch <= 65535. Every check runs before any launch, also on a
+ * host-only context; inputs are never written; scratch is stream-ordered (cudaMallocAsync on `stream`).
+ *
+ * Encode: Encoder.Embed / Encode with IsBatched (schemes/ckks/encoder.go:208-337): `values` holds n_values <= 2^log_slots complex128
+ * values per entry (16-byte aligned), zero-padded to the slots, 0 <= log_slots <= LogN - 1; IFFT, Complex128ToFixedPointCRT and
+ * rlwe.NTTSparseAndMontgomery into out_q (level_q + 1 rows) and, when level_p >= 0, out_p (level_p + 1 rows; the ringqp.Poly of a
+ * linear-transformation diagonal). Without LGPU_ENC_NTT the words are the reference's literal ones (possibly q, or an unreduced
+ * c < 2^61); the coefficient-domain case with slots < N/2 is rejected (the reference's spreading loop, core/rlwe/utils.go:234-241,
+ * has no defined output). With LGPU_ENC_COEFFS (encoder.go:156-189): n_values <= N float64 values, Float64ToFixedPointCRT, NTT when
+ * LGPU_ENC_NTT, level_p = -1; log_slots, rot_group and roots are unused. Values must be finite.
+ *
+ * Decode: Encoder.DecodePublic (encoder.go:497-762) of `batch` plaintexts pt [level + 1][N]: INTT when LGPU_ENC_NTT (NTT-domain words
+ * canonical), then polyToComplexNoCRT (level 0) / polyToComplexCRT, the forward special FFT and, for logprec != 0 (an integer in
+ * [-1022, 1023]), math.Round(x 2^logprec) / 2^logprec per part; `values` receives 2^log_slots complex128 per entry (16-byte aligned).
+ * With LGPU_ENC_COEFFS: polyToFloatNoCRT / polyToFloatCRT into N float64 per entry, no FFT, logprec unused. Q_level up to 4096 bits. */
+#define LGPU_ENC_NTT 1
+#define LGPU_ENC_MONTGOMERY 2
+#define LGPU_ENC_COEFFS 4
+int lgpu_ckks_encode(lgpu_ctx* ctx, const double* values, int n_values, int log_slots, double scale, int flags, const int64_t* rot_group,
+                     const double* roots, int level_q, uint64_t* out_q, int level_p, uint64_t* out_p, int batch, size_t values_stride,
+                     size_t out_q_stride, size_t out_p_stride, void* stream);
+int lgpu_ckks_decode(lgpu_ctx* ctx, const uint64_t* pt, int level, int log_slots, double scale, int flags, double logprec,
+                     const int64_t* rot_group, const double* roots, double* values, int batch, size_t pt_stride, size_t values_stride,
+                     void* stream);
 
 /* ---- wire format -> device (the reference's WriteTo / ReadFrom byte streams, little-endian uint64 words) ------------------
  * ring.Poly (ring/poly.go:132-179): rows, then per row {len, len words}. */

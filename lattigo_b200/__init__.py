@@ -15,3 +15,4 @@ from . import wire  # noqa: F401,E402
 from . import rgsw  # noqa: F401,E402
 from . import encryptor  # noqa: F401,E402
 from . import ckks_fft  # noqa: F401,E402
+from .encoder import Encoder  # noqa: F401,E402

@@ -102,6 +102,8 @@ def lib():
             "lgpu_blind_rotate_core": [vp, vp, i, vp, i, vp, vp, vp, i, vp],
             "lgpu_blind_rotation_evaluate": [vp, vp, vp, i, i, vp, i, vp, vp, vp, i, vp, i, i, vp, i, vp],
             "lgpu_ckks_special_fft": [vp, vp, i, i, vp, vp, i, i, z, vp],
+            "lgpu_ckks_encode": [vp, vp, i, i, c.c_double, i, vp, vp, i, vp, i, vp, i, z, z, z, vp],
+            "lgpu_ckks_decode": [vp, vp, i, i, c.c_double, i, c.c_double, vp, vp, vp, i, z, z, vp],
             "lgpu_poly_load": [vp, vp, z, vp, i, vp, vp, vp],
             "lgpu_poly_store": [vp, vp, i, vp, z, vp, vp],
             "lgpu_gadget_ct_load": [vp, vp, z, vp, z, vp, vp],
