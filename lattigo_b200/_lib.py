@@ -150,6 +150,18 @@ class GaloisKeysStruct(ctypes.Structure):
     _fields_ = [("n_keys", ctypes.c_int), ("gal_els", ctypes.POINTER(ctypes.c_uint64)), ("keys", ctypes.POINTER(GadgetCtStruct))]
 
 
+class GaloisKeys:
+    """The lgpu_galois_keys view of {galEl: GadgetCiphertext}. gks keeps its two host arrays alive (ctypes holds what a struct field
+    points to), but it also points into the keys' device tensors: whoever holds gks holds `keys` for as long."""
+
+    def __init__(self, keys):
+        self.keys = dict(keys)
+        els = list(self.keys)
+        self._els = (ctypes.c_uint64 * max(1, len(els)))(*els)
+        self._structs = (GadgetCtStruct * max(1, len(els)))(*[self.keys[g].struct for g in els])
+        self.gks = GaloisKeysStruct(len(els), self._els, self._structs)
+
+
 def check(rc):
     if rc != 0:
         raise LgpuError(lib().lgpu_last_error().decode())

@@ -333,19 +333,6 @@ struct lgpu_bgv {
 
 using namespace lgpu;
 
-static int bgv_gct(const lgpu_gadget_ct* e, GadgetCt& g) {
-    REQUIRE(e && e->data, "null relinearization key");
-    REQUIRE_ALIGNED(AL(e->data));
-    g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-    g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    return 0;
-}
-
-static bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes) {
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + bbytes && y < x + abytes;
-}
-
 extern "C" {
 
 int lgpu_bgv_create(lgpu_ctx* ctx, uint64_t t, const uint64_t* qmul, int nqmul, lgpu_bgv** out) {
@@ -429,7 +416,7 @@ int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const
     REQUIRE(out_is_a || !overlaps(ct_out, out_bytes, ct_a, in_bytes), "ct_out overlaps ct_a (only ct_out == ct_a without rescale is allowed)");
     REQUIRE((out_is_a && ct_a == ct_b) || !overlaps(ct_out, out_bytes, ct_b, in_bytes), "ct_out overlaps ct_b");
     GadgetCt g;
-    if (bgv_gct(rlk, g)) return -1;
+    if (to_gadget_ct(rlk, g, "null relinearization key")) return -1;
     if (check_evk(&c, level, g)) return -1;
     const cudaStream_t st = (cudaStream_t)stream;
     const u64* A = (const u64*)ct_a;

@@ -27,7 +27,6 @@
 #include <vector>
 #include "capi_common.h"
 #include "composite.h"
-#include "lintrans.h"
 #include "modarith.cuh"
 #include "ntt_arith.cuh"
 #include "xpow.cuh"
@@ -241,14 +240,6 @@ __global__ void __launch_bounds__(256) br_init_kernel(const LimbConst* limbs, co
     o[cs + i] = 0;
 }
 
-static int to_gct_br(const lgpu_gadget_ct* e, GadgetCt& g) {
-    REQUIRE(e && e->data, "null evaluation key");
-    REQUIRE_ALIGNED(AL(e->data));
-    g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-    g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    return 0;
-}
-
 static KeyDesc key_desc(const Ctx& c, const GadgetCt& g, u64 gal_el) {
     return KeyDesc{g.data, gal_el, (unsigned)((g.levelQ + 1 + g.levelP + 1) * (size_t)c.N), g.pw2_sizes ? g.pw2_sizes[0] : 1, g.pw2, 0};
 }
@@ -289,14 +280,14 @@ extern "C" int lgpu_blind_rotation_evaluate(lgpu_ctx* ctx, lgpu_ctx* ctx_lwe, co
     }
     REQUIRE_ALIGNED(AL(ct_lwe) && AL(ct_out));
     GadgetCt g0;
-    if (to_gct_br(&brk0[0], g0)) return -1;
+    if (to_gadget_ct(&brk0[0], g0)) return -1;
     const int level = g0.levelQ;
     REQUIRE(level >= 0 && level < c.nQ, "blind-rotation key level out of range");
     std::vector<KeyDesc> kd(2 * (size_t)n_lwe);
     for (int comp = 0; comp < 2; comp++) {
         for (int j = 0; j < n_lwe; j++) {
             GadgetCt g;
-            if (to_gct_br(comp ? &brk1[j] : &brk0[j], g)) return -1;
+            if (to_gadget_ct(comp ? &brk1[j] : &brk0[j], g)) return -1;
             REQUIRE(g.levelQ == g0.levelQ && g.levelP == g0.levelP && g.pw2 == g0.pw2,
                     "blind-rotation keys must share their levels and BaseTwoDecomposition");
             if (check_evk(&c, level, g)) return -1;
@@ -306,10 +297,7 @@ extern "C" int lgpu_blind_rotation_evaluate(lgpu_ctx* ctx, lgpu_ctx* ctx_lwe, co
     bool fused = level == 0 && g0.levelP == -1 && g0.pw2 >= 1 && g0.pw2 <= 62 && c.logN >= kFusedMinLogN && c.logN <= kFusedMaxLogN;
     // the automorphism keys Algorithm 3 can reach: GaloisElement(1..window) and NthRoot - GaloisGen (keys.go:94-101)
     GaloisKeySet ks;
-    REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
-    ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
-    ks.keys.resize(ks.n);
-    for (int i = 0; i < ks.n; i++) if (to_gct_br(&gks->keys[i], ks.keys[i])) return -1;
+    if (to_galois_keys(gks, ks)) return -1;
     std::vector<u64> need;
     for (int v = 1; v <= window_size && v <= c.N; v++) {
         const u64 g = galois_element(&c, v);

@@ -31,6 +31,29 @@ int make_rowmap_single(const Ctx& c, int ring, int limb, RowMap& rm) {
     rm.drow[0] = 0;
     return 0;
 }
+
+int to_gadget_ct(const lgpu_gadget_ct* e, GadgetCt& g, const char* null_msg) {
+    REQUIRE(e && e->data, null_msg);
+    REQUIRE_ALIGNED(AL(e->data));
+    g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
+    g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
+    return 0;
+}
+
+int to_galois_keys(const lgpu_galois_keys* gks, GaloisKeySet& ks) {
+    REQUIRE(gks, "null Galois key set");
+    REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
+    ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
+    ks.keys.resize(ks.n);
+    for (int i = 0; i < ks.n; i++)
+        if (to_gadget_ct(&gks->keys[i], ks.keys[i])) return -1;
+    return 0;
+}
+
+bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes) {
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + bbytes && y < x + abytes;
+}
 }  // namespace lgpu
 
 extern "C" {

@@ -12,13 +12,6 @@ using namespace lgpu;
 
 static inline cudaStream_t S(void* stream) { return (cudaStream_t)stream; }
 
-static int to_gct(const lgpu_gadget_ct* e, GadgetCt& g) {
-    REQUIRE(e && e->data, "null evaluation key");
-    REQUIRE_ALIGNED(AL(e->data));
-    g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-    g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    return 0;
-}
 static int check_levels(const Ctx& c, int lq, int lp, bool needP) {
     REQUIRE(lq >= 0 && lq < c.nQ, "levelQ out of range");
     if (needP) REQUIRE(lp >= 0 && lp < c.nP, "levelP out of range");
@@ -130,7 +123,7 @@ int lgpu_gadget_product(lgpu_ctx* ctx, int lq, const uint64_t* cx, const lgpu_ga
     REQUIRE(cx && ct0 && ct1, "null polynomial");
     REQUIRE_ALIGNED(AL(cx) && AL(ct0) && AL(ct1) && ((scx | sct) & 1) == 0);
     GadgetCt g;
-    if (to_gct(evk, g)) return -1;
+    if (to_gadget_ct(evk, g)) return -1;
     lq = std::min(lq, g.levelQ);   // core/rlwe/evaluator_gadget_product.go:18
     const size_t N = ctx->c.N;
     return gadget_product(&ctx->c, lq, CSpan{(const u64*)cx, N, scx}, g, Span{(u64*)ct0, N, sct}, Span{(u64*)ct1, N, sct}, batch, S(stream));
@@ -141,7 +134,7 @@ int lgpu_gadget_product_lazy(lgpu_ctx* ctx, int lq, const uint64_t* cx, const lg
     REQUIRE(cx && a0q && a1q, "null polynomial");
     REQUIRE_ALIGNED(AL(cx) && AL(a0q) && AL(a0p) && AL(a1q) && AL(a1p) && ((scx | sq | sp) & 1) == 0);
     GadgetCt g;
-    if (to_gct(evk, g)) return -1;
+    if (to_gadget_ct(evk, g)) return -1;
     REQUIRE(g.levelP < 0 || (a0p && a1p), "null P accumulator");
     const size_t N = ctx->c.N;
     return gadget_product_lazy(&ctx->c, lq, CSpan{(const u64*)cx, N, scx}, g, make_acc((u64*)a0q, (u64*)a0p, (u64*)a1q, (u64*)a1p, N, sq, sp), batch, S(stream));
@@ -178,7 +171,7 @@ int lgpu_gadget_product_hoisted(lgpu_ctx* ctx, int lq, const uint64_t* decomp, c
     REQUIRE(decomp && ct0 && ct1, "null polynomial");
     REQUIRE_ALIGNED(AL(decomp) && AL(ct0) && AL(ct1) && (sct & 1) == 0);
     GadgetCt g;
-    if (to_gct(evk, g)) return -1;
+    if (to_gadget_ct(evk, g)) return -1;
     const size_t N = ctx->c.N;
     return gadget_product_hoisted(&ctx->c, lq, (const u64*)decomp, g, Span{(u64*)ct0, N, sct}, Span{(u64*)ct1, N, sct}, batch, S(stream));
 }
@@ -188,7 +181,7 @@ int lgpu_gadget_product_hoisted_lazy(lgpu_ctx* ctx, int lq, const uint64_t* deco
     REQUIRE(decomp && a0q && a0p && a1q && a1p, "null polynomial");
     REQUIRE_ALIGNED(AL(decomp) && AL(a0q) && AL(a0p) && AL(a1q) && AL(a1p) && ((sq | sp) & 1) == 0);
     GadgetCt g;
-    if (to_gct(evk, g)) return -1;
+    if (to_gadget_ct(evk, g)) return -1;
     const size_t N = ctx->c.N;
     return gadget_product_hoisted_lazy(&ctx->c, lq, (const u64*)decomp, g, make_acc((u64*)a0q, (u64*)a0p, (u64*)a1q, (u64*)a1p, N, sq, sp), batch, S(stream));
 }
@@ -198,7 +191,7 @@ int lgpu_evaluator_automorphism(lgpu_ctx* ctx, int level, const uint64_t* ct_in,
     REQUIRE(ct_in && ct_out, "null ciphertext");
     REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
     GadgetCt g;
-    if (to_gct(gk, g)) return -1;
+    if (to_gadget_ct(gk, g)) return -1;
     REQUIRE(level >= 0 && level <= g.levelQ && level < ctx->c.nQ, "level out of range");
     const size_t N = ctx->c.N, nq = level + 1, cs = 2 * nq * N;
     const u64* in = (const u64*)ct_in;
@@ -211,7 +204,7 @@ int lgpu_evaluator_relinearize(lgpu_ctx* ctx, int level, const uint64_t* ct_in, 
     REQUIRE(ct_in && ct_out, "null ciphertext");
     REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
     GadgetCt g;
-    if (to_gct(rlk, g)) return -1;
+    if (to_gadget_ct(rlk, g)) return -1;
     REQUIRE(level >= 0 && level <= g.levelQ && level < ctx->c.nQ, "level out of range");
     const size_t N = ctx->c.N, nq = level + 1;
     const u64* in = (const u64*)ct_in;
@@ -227,7 +220,7 @@ int lgpu_ckks_mulrelin_rescale_batch(lgpu_ctx* ctx, int level, const uint64_t* c
     REQUIRE_ALIGNED(AL(ct_a) && AL(ct_b) && AL(ct_out));
     REQUIRE(batch >= 1, "batch must be >= 1");
     GadgetCt g;
-    if (to_gct(rlk, g)) return -1;
+    if (to_gadget_ct(rlk, g)) return -1;
     return ckks_mulrelin_rescale(&ctx->c, level, (const u64*)ct_a, (const u64*)ct_b, g, nb_rescales, (u64*)ct_out, batch, S(stream));
 }
 
@@ -238,7 +231,7 @@ int lgpu_ckks_mulrelin_rescale_batch_host(lgpu_ctx* ctx, int level, const uint64
     REQUIRE(ct_a_host && ct_b_host && ct_out_host, "null ciphertext");
     REQUIRE(batch >= 1, "batch must be >= 1");
     GadgetCt g;
-    if (to_gct(rlk, g)) return -1;
+    if (to_gadget_ct(rlk, g)) return -1;
     const Ctx& c = ctx->c;
     REQUIRE(level >= 0 && level < c.nQ && nb_rescales >= 0 && nb_rescales <= level, "level out of range");
     if (chunk <= 0) chunk = 2;   // short chunks shrink the pipeline's head and tail (H100: profiles/h100_switch_ab.md)

@@ -10,14 +10,6 @@ using namespace lgpu;
 
 static inline cudaStream_t S(void* stream) { return (cudaStream_t)stream; }
 
-static int to_gct3(const lgpu_gadget_ct* e, GadgetCt& g) {
-    REQUIRE(e && e->data, "null evaluation key");
-    REQUIRE_ALIGNED(AL(e->data));
-    g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-    g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    return 0;
-}
-
 extern "C" {
 
 uint64_t lgpu_galois_element(lgpu_ctx* ctx, long long k) {
@@ -34,13 +26,8 @@ int lgpu_lintrans_evaluate_many(lgpu_ctx* ctx, int level_in, const uint64_t* ct_
     REQUIRE_ALIGNED(AL(ct_in));
     GaloisKeySet ks;
     if (gks) {
-        REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
-        ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
-        ks.keys.resize(ks.n);
-        for (int i = 0; i < ks.n; i++) {
-            if (to_gct3(&gks->keys[i], ks.keys[i])) return -1;
-            REQUIRE(ks.keys[i].pw2 == 0, "hoisted linear transformations need keys with BaseTwoDecomposition = 0");
-        }
+        if (to_galois_keys(gks, ks)) return -1;
+        for (const GadgetCt& k : ks.keys) REQUIRE(k.pw2 == 0, "hoisted linear transformations need keys with BaseTwoDecomposition = 0");
     }
     std::vector<LinTransView> mv(n_mats);
     for (int i = 0; i < n_mats; i++) {
@@ -63,7 +50,7 @@ int lgpu_rgsw_external_product(lgpu_ctx* ctx, const uint64_t* ct_in, int level_i
     REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
     REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
     GadgetCt g0, g1;
-    if (to_gct3(rgsw0, g0) || to_gct3(rgsw1, g1)) return -1;
+    if (to_gadget_ct(rgsw0, g0) || to_gadget_ct(rgsw1, g1)) return -1;
     REQUIRE(g0.levelQ >= 0 && g0.levelQ <= level_in && g0.levelQ <= level_out, "RGSW ciphertext level above the RLWE ciphertexts' level");
     const size_t N = ctx->c.N, ci = (size_t)(level_in + 1) * N, co = (size_t)(level_out + 1) * N;
     const u64* in = (const u64*)ct_in;
@@ -106,10 +93,7 @@ int lgpu_blind_rotate_core(lgpu_ctx* ctx, const uint64_t* a_host, int n_lwe, uin
         sets[has[ai] ? dlog[ai] : 0].push_back(i);
     }
     GaloisKeySet ks;
-    REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
-    ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
-    ks.keys.resize(ks.n);
-    for (int i = 0; i < ks.n; i++) if (to_gct3(&gks->keys[i], ks.keys[i])) return -1;
+    if (to_galois_keys(gks, ks)) return -1;
     const size_t nq = level + 1, cs = nq * (size_t)N;
     u64* A = (u64*)acc;
     cudaStream_t st = S(stream);
@@ -126,7 +110,7 @@ int lgpu_blind_rotate_core(lgpu_ctx* ctx, const uint64_t* a_host, int n_lwe, uin
             if (v != 0) { if (automorph(v)) return -1; v = 0; }
             for (int j : it->second) {
                 GadgetCt g0, g1;
-                if (to_gct3(&brk0[j], g0) || to_gct3(&brk1[j], g1)) return -1;
+                if (to_gadget_ct(&brk0[j], g0) || to_gadget_ct(&brk1[j], g1)) return -1;
                 if (rgsw_external_product(&c, g0, g1, CSpan{A, (size_t)N, 2 * cs}, CSpan{A + cs, (size_t)N, 2 * cs}, Span{A, (size_t)N, 2 * cs},
                                           Span{A + cs, (size_t)N, 2 * cs}, 1, st)) return -1;
             }
@@ -159,20 +143,14 @@ int lgpu_evaluator_automorphism_hoisted_lazy(lgpu_ctx* ctx, int level_q, const u
     REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
     REQUIRE_ALIGNED(AL(ct0) && AL(decomp) && AL(out0q) && AL(out0p) && AL(out1q) && AL(out1p) && ((stride_ct | stride_q | stride_p) & 1) == 0);
     GadgetCt g;
-    if (to_gct3(gk, g)) return -1;
+    if (to_gadget_ct(gk, g)) return -1;
     const Ctx& c = ctx->c;
     REQUIRE(level_q >= 0 && level_q < c.nQ && level_q <= g.levelQ, "levelQ out of range");
     REQUIRE(g.levelP >= 0 && g.levelP < c.nP, "AutomorphismHoistedLazy requires a P ring");
     if (decomp_level_q < 0) decomp_level_q = level_q;
     const size_t N = c.N, nq = level_q + 1;
     // ctIn.Value[0] * P (ringQ.MulScalarBigint, evaluator_automorphism.go:150-156)
-    std::vector<u64> pq(nq);
-    for (size_t i = 0; i < nq; i++) {
-        const u64 q = c.Q[i];
-        u64 v = 1;
-        for (int j = 0; j <= g.levelP; j++) v = h_mulmod(v, c.P[j] % q, q);
-        pq[i] = h_mform(v, q);
-    }
+    const std::vector<u64> pq = p_mod_q_mont(&c, level_q, g.levelP);
     Scratch buf;
     if (buf.alloc((size_t)batch * nq * N, S(stream))) return -1;
     if (launch_vecop(&c, rows_range(0, 0, (int)nq), LGPU_OP_MULSCALARMONTGOMERY, CSpan{(const u64*)ct0, N, stride_ct}, CSpan{nullptr, 0, 0},

@@ -1,8 +1,9 @@
-// capi_common.h -- shared by the extern "C" translation units (capi.cu, capi2.cu, ringmisc.cu): the opaque handle,
-// argument-check macros and the row-map helpers.
+// capi_common.h -- shared by the extern "C" translation units: the opaque handle, argument-check macros, the row-map helpers and
+// the conversions of the key structs of the public header.
 #pragma once
 #include <cstdint>
 #include "../../include/lattigo_b200.h"
+#include "composite.h"
 #include "engine.h"
 #include <nvtx3/nvToolsExt.h>
 
@@ -39,4 +40,10 @@ namespace lgpu {
 // rows 0..level of ring Q or P -> global limb indices (capi.cu)
 int make_rowmap(const Ctx& c, int ring, int level, RowMap& rm);
 int make_rowmap_single(const Ctx& c, int ring, int limb, RowMap& rm);
+// lgpu_gadget_ct -> GadgetCt: null key or data (null_msg), 16-byte alignment of the data, n_pw2_max <= 0 read as 1 (capi.cu)
+int to_gadget_ct(const lgpu_gadget_ct* e, GadgetCt& g, const char* null_msg = "null evaluation key");
+// lgpu_galois_keys -> GaloisKeySet: null set, null arrays for n_keys > 0, then every key through to_gadget_ct (capi.cu)
+int to_galois_keys(const lgpu_galois_keys* gks, GaloisKeySet& ks);
+// [a, a + abytes) and [b, b + bbytes) intersect
+bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes);
 }  // namespace lgpu

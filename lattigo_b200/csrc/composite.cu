@@ -19,6 +19,33 @@
 namespace lgpu {
 
 // ---------------------------------------------------------------------------------------------------------
+// host helpers
+// ---------------------------------------------------------------------------------------------------------
+u64 galois_element(const Ctx* c, long long k) {   // rlwe.Parameters.GaloisElement, core/rlwe/params.go:580-583 (GaloisGen = 5)
+    const u64 m = c->nthroot;
+    u64 e = (u64)k & (m - 1), base = 5 % m, r = 1;
+    while (e) { if (e & 1) r = r * base & (m - 1); base = base * base & (m - 1); e >>= 1; }
+    return r;
+}
+
+const GadgetCt* GaloisKeySet::find(u64 galEl) const {
+    for (int i = 0; i < n; i++) if (gal_els[i] == galEl) return &keys[i];
+    set_error("GaloisKey[" + std::to_string(galEl) + "] is missing");      // rlwe.EvaluationKeySet.GetGaloisKey
+    return nullptr;
+}
+
+std::vector<u64> p_mod_q_mont(const Ctx* c, int levelQ, int levelP) {
+    std::vector<u64> s(levelQ + 1);
+    for (int i = 0; i <= levelQ; i++) {
+        const u64 q = c->Q[i];
+        u64 v = 1;
+        for (int j = 0; j <= levelP; j++) v = h_mulmod(v, c->P[j] % q, q);
+        s[i] = h_mform(v, q);
+    }
+    return s;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // ModDown
 // ---------------------------------------------------------------------------------------------------------
 static int moddown_finish(const Ctx* c, bool toQ, int levelQ, int levelP, CSpan ext, CSpan p1, Span p2, int batch, cudaStream_t st) {
@@ -525,12 +552,7 @@ int gadget_product(const Ctx* c, int levelQ, CSpan cx, const GadgetCt& evk, Span
     const size_t N = c->N, nq = levelQ + 1, np = levelP + 1;
     Scratch buf;
     if (buf.alloc((size_t)batch * 2 * (nq + np) * N, st)) return -1;
-    AccSpans acc;
-    for (int k = 0; k < 2; k++) {
-        u64* base = buf.p + (size_t)k * batch * (nq + np) * N;
-        acc.q[k] = Span{base, N, (nq + np) * N};
-        acc.p[k] = Span{base + nq * N, N, (nq + np) * N};
-    }
+    const AccSpans acc = stacked_acc(buf.p, nq, np, N, batch);
     if (gadget_product_lazy(c, levelQ, cx, evk, acc, batch, st)) return -1;
     return evaluator_moddown_ntt(c, levelQ, levelP, acc, ct0, ct1, batch, st);
 }
@@ -549,16 +571,7 @@ int rgsw_external_product(const Ctx* c, const GadgetCt& rg0, const GadgetCt& rg1
     Scratch buf;
     const size_t per = (size_t)2 * batch * (nq + np) * N;
     if (buf.alloc(2 * per, st)) return -1;
-    auto stacked = [&](u64* base) {
-        AccSpans a;
-        for (int k = 0; k < 2; k++) {
-            u64* b = base + (size_t)k * batch * (nq + np) * N;
-            a.q[k] = Span{b, N, (nq + np) * N};
-            a.p[k] = Span{b + nq * N, N, (nq + np) * N};
-        }
-        return a;
-    };
-    AccSpans A = stacked(buf.p), B = stacked(buf.p + per);
+    const AccSpans A = stacked_acc(buf.p, nq, np, N, batch), B = stacked_acc(buf.p + per, nq, np, N, batch);
     if (levelP >= 1) {
         if (rg0.pw2 != 0) { set_error("RGSW external product: BaseTwoDecomposition != 0 requires levelP <= 0"); return -1; }
         if (gadget_product_multiple_p_lazy(c, levelQ, ct0, rg0, A, batch, st)) return -1;
@@ -630,12 +643,7 @@ int gadget_product_hoisted(const Ctx* c, int levelQ, const u64* decomp, const Ga
     const size_t N = c->N, nq = levelQ + 1, np = levelP + 1;
     Scratch buf;
     if (buf.alloc((size_t)batch * 2 * (nq + np) * N, st)) return -1;
-    AccSpans acc;
-    for (int k = 0; k < 2; k++) {
-        u64* base = buf.p + (size_t)k * batch * (nq + np) * N;
-        acc.q[k] = Span{base, N, (nq + np) * N};
-        acc.p[k] = Span{base + nq * N, N, (nq + np) * N};
-    }
+    const AccSpans acc = stacked_acc(buf.p, nq, np, N, batch);
     if (gadget_product_hoisted_lazy(c, levelQ, decomp, evk, acc, batch, st)) return -1;
     return evaluator_moddown_ntt(c, levelQ, levelP, acc, ct0, ct1, batch, st);
 }
@@ -780,12 +788,7 @@ int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_r
         const size_t np = rlk.levelP + 1;
         Scratch accb;
         if (accb.alloc((size_t)2 * batch * (nq + np) * N, st)) return -1;
-        AccSpans acc;
-        for (int k = 0; k < 2; k++) {
-            u64* base = accb.p + (size_t)k * batch * (nq + np) * N;
-            acc.q[k] = Span{base, N, (nq + np) * N};
-            acc.p[k] = Span{base + nq * N, N, (nq + np) * N};
-        }
+        const AccSpans acc = stacked_acc(accb.p, nq, np, N, batch);
         if (gadget_product_lazy(c, level, CSpan{d2, N, nq * N}, rlk, acc, batch, st)) return -1;
         // d0, d1 are consecutive [comp][batch][nq][N] blocks: out = d + ModDown(acc), in place
         if (moddown_ntt_fused(c, level, rlk.levelP, accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N, d0, (size_t)batch * nq * N, nq * N,

@@ -1,5 +1,6 @@
 // composite.h -- prototypes of composite.cu (multi-kernel operations of the hot path).
 #pragma once
+#include <vector>
 #include "engine.h"
 
 namespace lgpu {
@@ -18,6 +19,12 @@ struct GadgetCt {          // device-side view of a rlwe.GadgetCiphertext (mirro
 struct AccSpans {  // the four accumulator polynomials of a ctQP: [comp].Q (levelQ+1 rows) and [comp].P (levelP+1 rows)
     Span q[2];
     Span p[2];
+};
+struct GaloisKeySet {        // the GaloisKeys map of rlwe.MemEvaluationKeySet, core/rlwe/evaluationkeyset.go
+    int n = 0;
+    const u64* gal_els = nullptr;
+    std::vector<GadgetCt> keys;
+    const GadgetCt* find(u64 galEl) const;   // nullptr + error "GaloisKey[..] is missing"
 };
 
 struct Scratch {
@@ -45,6 +52,20 @@ inline RowMap rows_qp(const Ctx* c, int nq, int np) {
     for (int j = 0; j < np; j++) { rm.limb[nq + j] = (unsigned char)(c->nQ + j); rm.drow[nq + j] = (unsigned char)(nq + j); }
     return rm;
 }
+// the accumulators of a [comp][batch][nq + np][N] block: each element's np P rows right after its nq Q rows
+inline AccSpans stacked_acc(u64* base, size_t nq, size_t np, size_t N, int batch) {
+    AccSpans a;
+    for (int k = 0; k < 2; k++) {
+        u64* b = base + (size_t)k * batch * (nq + np) * N;
+        a.q[k] = Span{b, N, (nq + np) * N};
+        a.p[k] = Span{b + nq * N, N, (nq + np) * N};
+    }
+    return a;
+}
+
+u64 galois_element(const Ctx* c, long long k);
+// p * P_levelP mod q_i in Montgomery form, i <= levelQ: the per-limb scalars of ringQ.MulScalarBigint(., P, .)
+std::vector<u64> p_mod_q_mont(const Ctx* c, int levelQ, int levelP);
 
 int base_rns_decomposition_vector_size(int levelQ, int levelP);
 int moddown_qp_to_q(const Ctx* c, int levelQ, int levelP, CSpan p1Q, CSpan p1P, Span p2Q, int batch, cudaStream_t st);

@@ -380,10 +380,11 @@ int lgpu_encrypt_zero_sk(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t
 int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t* sk_out, lgpu_gadget_ct* evk, const int64_t* e, void* stream) {
     REQUIRE_DEVICE(ctx);
     REQUIRE(sk_in && sk_out && evk && evk->data && e, "null argument");
-    REQUIRE_ALIGNED(AL(evk->data));
-    REQUIRE(evk->level_q == ctx->c.nQ - 1 && evk->level_p == ctx->c.nP - 1, "evaluation keys are generated at the maximum levels");
-    return gen_evaluation_key(&ctx->c, evk->base_two_decomposition, (const u64*)sk_in, (const u64*)sk_out, (u64*)evk->data, evk->n_digits,
-                              evk->n_pw2_max > 0 ? evk->n_pw2_max : 1, evk->pw2_sizes, (const long long*)e, (cudaStream_t)stream);
+    GadgetCt g;
+    if (to_gadget_ct(evk, g)) return -1;
+    REQUIRE(g.levelQ == ctx->c.nQ - 1 && g.levelP == ctx->c.nP - 1, "evaluation keys are generated at the maximum levels");
+    return gen_evaluation_key(&ctx->c, g.pw2, (const u64*)sk_in, (const u64*)sk_out, (u64*)evk->data, g.ndigits, g.npw2max, g.pw2_sizes,
+                              (const long long*)e, (cudaStream_t)stream);
 }
 
 }  // extern "C"

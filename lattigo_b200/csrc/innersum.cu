@@ -81,8 +81,6 @@ int copy_ct(const Ctx* c, int nq, Ct in, Ct out, int nb, cudaStream_t st) {
     return 0;
 }
 
-u64 gal_for(const Ctx* c, long long k) { return galois_element(c, k); }
-
 // The schedule of PartialTracesSum (inner_sum.go:217-283) for n >= 2: per iteration i < top bit of n, the optional lazy term
 // (k = (n - (n mod 2^(i+1))) * offset, when bit i of n is set) and the doubling rotation 2^i * offset.
 struct PtsStep { bool lazy; long long k; long long dbl; };
@@ -103,7 +101,7 @@ std::vector<u64> trace_elements(const Ctx* c, int log_n) {
     std::vector<u64> g;
     const int gap_log = c->logN - log_n - 1 + (log_n == 0 ? 1 : 0);
     if (gap_log <= 0) return g;
-    for (int i = log_n; i < c->logN - 1; i++) g.push_back(gal_for(c, 1ll << i));
+    for (int i = log_n; i < c->logN - 1; i++) g.push_back(galois_element(c, 1ll << i));
     if (log_n == 0) g.push_back(c->nthroot - 1);
     return g;
 }
@@ -150,21 +148,8 @@ int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, co
     for (int s = 0; s <= d; s++) X[s] = bufs[tag[s]];
     if (copy_in && copy_ct(c, nq, in, X[0], nb, st)) return -1;
     if (!is_ntt && ntt_ct(c, false, nq, in, X[0], nb, st)) return -1;
-    AccSpans acc;
-    for (int k = 0; k < 2; k++) {
-        u64* b = accb + (size_t)k * nb * (nq + np) * N;
-        acc.q[k] = Span{b, N, (nq + np) * N};
-        acc.p[k] = Span{b + (size_t)nq * N, N, (nq + np) * N};
-    }
-    const std::vector<u64> pq = [&] {
-        std::vector<u64> v(nq);
-        for (int i = 0; i < nq; i++) {
-            u64 x = 1;
-            for (int j = 0; j <= levelP; j++) x = h_mulmod(x, c->P[j] % c->Q[i], c->Q[i]);
-            v[i] = h_mform(x, c->Q[i]);
-        }
-        return v;
-    }();
+    const AccSpans acc = stacked_acc(accb, nq, np, N, nb);
+    const std::vector<u64> pq = p_mod_q_mont(c, level, levelP);
     bool first = true;
     for (int i = 0; i < d; i++) {
         const Ct x = X[i];
@@ -174,14 +159,14 @@ int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, co
             // accQP (+)= AutomorphismHoistedLazy(ctInNTT, k); P * ctInNTT[0] is its Q-row addend (evaluator_automorphism.go:150-156)
             if (launch_vecop(c, rows_range(0, 0, nq), LGPU_OP_MULSCALARMONTGOMERY, CSpan{x.p, N, 2 * x.cs}, CSpan{nullptr, 0, 0}, Span{c0p, N, (size_t)nq * N},
                              nb, pq.data(), nullptr, 0, 0, c->N, st)) return -1;
-            if (automorphism_hoisted_lazy(c, level, CSpan{c0p, N, (size_t)nq * N}, decomp, level, gal_for(c, sched[i].k), *lazy_keys[i], acc, nb, st, !first))
+            if (automorphism_hoisted_lazy(c, level, CSpan{c0p, N, (size_t)nq * N}, decomp, level, galois_element(c, sched[i].k), *lazy_keys[i], acc, nb, st, !first))
                 return -1;
             first = false;
         }
         // ctInNTT = ctInNTT + AutomorphismHoisted(ctInNTT, 2^i * offset)
         if (gadget_product_hoisted(c, level, decomp, *dbl_keys[i], Span{t, N, (size_t)nq * N}, Span{t + (size_t)nb * nq * N, N, (size_t)nq * N}, nb, st))
             return -1;
-        if (auto_add(c, nq, x, t, nb, X[i + 1], gal_for(c, sched[i].dbl), st)) return -1;
+        if (auto_add(c, nq, x, t, nb, X[i + 1], galois_element(c, sched[i].dbl), st)) return -1;
     }
     if (n & (n - 1)) {
         // opOut = ModDown(accQP) + ctInNTT (:256-263); X[d] is `out`, so the addend is read and written in place
@@ -231,27 +216,6 @@ int trace_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int log_n, const st
     return 0;
 }
 
-bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes) {
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + bbytes && y < x + abytes;
-}
-
-int to_keyset(const lgpu_galois_keys* gks, GaloisKeySet& ks) {
-    REQUIRE(gks, "null Galois key set");
-    REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
-    ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
-    ks.keys.resize(ks.n);
-    for (int i = 0; i < ks.n; i++) {
-        const lgpu_gadget_ct* e = &gks->keys[i];
-        REQUIRE(e->data, "null evaluation key");
-        REQUIRE_ALIGNED(AL(e->data));
-        GadgetCt& g = ks.keys[i];
-        g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-        g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    }
-    return 0;
-}
-
 // every key the call will use, looked up and checked before any device work (the reference fails at the first missing key instead)
 int lookup(const Ctx* c, const GaloisKeySet& ks, int level, u64 g, bool max_levelP, const GadgetCt*& out) {
     out = ks.find(g);
@@ -288,7 +252,7 @@ int lgpu_evaluator_partial_traces_sum(lgpu_ctx* ctx, int level, const uint64_t* 
     GaloisKeySet ks;
     if (n >= 2) {
         REQUIRE(c.nP >= 1, "PartialTracesSum requires a P ring");
-        if (to_keyset(gks, ks)) return -1;
+        if (to_galois_keys(gks, ks)) return -1;
         for (const PtsStep& s : pts_schedule(offset, n)) {
             const GadgetCt* g = nullptr;
             if (s.lazy && lookup(&c, ks, level, galois_element(&c, s.k), true, g)) return -1;
@@ -329,7 +293,7 @@ int lgpu_evaluator_trace(lgpu_ctx* ctx, int level_in, const uint64_t* ct_in, int
     GaloisKeySet ks;
     if (!els.empty()) {
         REQUIRE(c.nP >= 1, "Trace requires a P ring");
-        if (to_keyset(gks, ks)) return -1;
+        if (to_galois_keys(gks, ks)) return -1;
         for (u64 g : els) {
             const GadgetCt* k = nullptr;
             if (lookup(&c, ks, level, g, false, k)) return -1;

@@ -167,41 +167,6 @@ __global__ void __launch_bounds__(256) lt_hoisted_auto_kernel(HoistParams p) {
 // ---------------------------------------------------------------------------------------------------------------------
 // host helpers
 // ---------------------------------------------------------------------------------------------------------------------
-u64 galois_element(const Ctx* c, long long k) {   // rlwe.Parameters.GaloisElement, core/rlwe/params.go:580-583 (GaloisGen = 5)
-    const u64 m = c->nthroot;
-    u64 e = (u64)k & (m - 1), base = 5 % m, r = 1;
-    while (e) { if (e & 1) r = r * base & (m - 1); base = base * base & (m - 1); e >>= 1; }
-    return r;
-}
-
-const GadgetCt* GaloisKeySet::find(u64 galEl) const {
-    for (int i = 0; i < n; i++) if (gal_els[i] == galEl) return &keys[i];
-    set_error("GaloisKey[" + std::to_string(galEl) + "] is missing");      // rlwe.EvaluationKeySet.GetGaloisKey
-    return nullptr;
-}
-
-static AccSpans stacked_acc(u64* base, size_t nq, size_t np, size_t N, int batch) {   // [comp][batch][nq + np][N]
-    AccSpans a;
-    for (int k = 0; k < 2; k++) {
-        u64* b = base + (size_t)k * batch * (nq + np) * N;
-        a.q[k] = Span{b, N, (nq + np) * N};
-        a.p[k] = Span{b + nq * N, N, (nq + np) * N};
-    }
-    return a;
-}
-
-// p * P_levelP mod q_i in Montgomery form, i <= levelQ: the per-limb scalars of ringQ.MulScalarBigint(., P, .)
-static std::vector<u64> p_mod_q_mont(const Ctx* c, int levelQ, int levelP) {
-    std::vector<u64> s(levelQ + 1);
-    for (int i = 0; i <= levelQ; i++) {
-        const u64 q = c->Q[i];
-        u64 v = 1;
-        for (int j = 0; j <= levelP; j++) v = h_mulmod(v, c->P[j] % q, q);
-        s[i] = h_mform(v, q);
-    }
-    return s;
-}
-
 // Evaluator.AutomorphismHoistedLazy (core/rlwe/evaluator_automorphism.go:107-165), NTT-domain branch: out = pi_galEl(
 // <decomp, gk> + (P * ct0, 0)) mod QP. ct0P = P * ct0 (rows [0, levelQ], canonical).
 int check_gk(const Ctx* c, int levelQ, const GadgetCt& gk) {

@@ -1,4 +1,4 @@
-// lintrans.h -- host-side views used by lintrans.cu (mirrors of lgpu_lintrans / lgpu_galois_keys of the public header).
+// lintrans.h -- host-side view used by lintrans.cu (mirror of lgpu_lintrans of the public header).
 #pragma once
 #include <map>
 #include <vector>
@@ -11,14 +11,7 @@ struct LinTransView {        // lintrans.LinearTransformation, circuits/common/l
     const int* diag_index;   // host: keys of Vec
     const u64* const* diag;  // host array of device pointers: (level_q+1) Q rows then (level_p+1) P rows, NTT + Montgomery
 };
-struct GaloisKeySet {        // the GaloisKeys map of rlwe.MemEvaluationKeySet, core/rlwe/evaluationkeyset.go
-    int n = 0;
-    const u64* gal_els = nullptr;
-    std::vector<GadgetCt> keys;
-    const GadgetCt* find(u64 galEl) const;   // nullptr + error "GaloisKey[..] is missing"
-};
 
-u64 galois_element(const Ctx* c, long long k);
 void bsgs_index(const LinTransView& m, std::map<int, std::vector<int>>& index, std::vector<int>& rotN1, std::vector<int>& rotN2);
 // accumulate: out = CRed(out + result) (needs QP-stacked outputs: out.p[k] right after the nq rows of out.q[k], one batch stride)
 int automorphism_hoisted_lazy(const Ctx* c, int levelQ, CSpan ct0P, const u64* decomp, int decomp_levelQ, u64 galEl, const GadgetCt& gk,

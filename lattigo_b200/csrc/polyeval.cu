@@ -355,10 +355,7 @@ extern "C" int lgpu_ckks_polynomial_evaluate(lgpu_ctx* ctx, int level, const uin
     bool needs_rlk = false;
     for (int i = 0; i < prog->n_ops; i++) needs_rlk |= prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN;
     if (needs_rlk) {
-        REQUIRE(rlk && rlk->data, "null relinearization key");
-        REQUIRE_ALIGNED(AL(rlk->data));
-        g.data = (const u64*)rlk->data; g.levelQ = rlk->level_q; g.levelP = rlk->level_p; g.pw2 = rlk->base_two_decomposition;
-        g.ndigits = rlk->n_digits; g.npw2max = rlk->n_pw2_max > 0 ? rlk->n_pw2_max : 1; g.pw2_sizes = rlk->pw2_sizes;
+        if (to_gadget_ct(rlk, g, "null relinearization key")) return -1;
         for (int i = 0; i < prog->n_ops; i++)
             if ((prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN) && check_evk(&c, prog->ops[i].level, g)) return -1;
     }

@@ -16,7 +16,6 @@
 #include <vector>
 #include "capi_common.h"
 #include "composite.h"
-#include "lintrans.h"
 #include "modarith.cuh"
 #include "xpow.cuh"
 
@@ -156,27 +155,6 @@ int log2_nthroot_half(const Ctx* c) {
     return lg;
 }
 u64 shoup(u64 w, u64 q) { return (u64)(((unsigned __int128)w << 64) / q); }
-
-bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes) {
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + bbytes && y < x + abytes;
-}
-
-int to_keyset(const lgpu_galois_keys* gks, GaloisKeySet& ks) {
-    REQUIRE(gks, "null Galois key set");
-    REQUIRE(gks->n_keys >= 0 && (gks->n_keys == 0 || (gks->gal_els && gks->keys)), "null Galois key arrays");
-    ks.n = gks->n_keys; ks.gal_els = (const u64*)gks->gal_els;
-    ks.keys.resize(ks.n);
-    for (int i = 0; i < ks.n; i++) {
-        const lgpu_gadget_ct* e = &gks->keys[i];
-        REQUIRE(e->data, "null evaluation key");
-        REQUIRE_ALIGNED(AL(e->data));
-        GadgetCt& g = ks.keys[i];
-        g.data = (const u64*)e->data; g.levelQ = e->level_q; g.levelP = e->level_p; g.pw2 = e->base_two_decomposition;
-        g.ndigits = e->n_digits; g.npw2max = e->n_pw2_max > 0 ? e->n_pw2_max : 1; g.pw2_sizes = e->pw2_sizes;
-    }
-    return 0;
-}
 
 // a key gadget_product accepts at `level` (the reference's Automorphism -> GadgetProduct), looked up before any device work
 int lookup(const Ctx* c, const GaloisKeySet& ks, int level, u64 g, const GadgetCt*& out) {
@@ -436,7 +414,7 @@ int lgpu_ring_packing_expand(lgpu_ctx* ctx, int level, const uint64_t* ct_in, in
     const size_t ctb = (size_t)2 * (level + 1) * c.N * 8;
     REQUIRE(!overlaps(ct_out, ctb * batch * (c.N >> log_gap), ct_in, ctb * batch), "ct_out overlaps ct_in");
     GaloisKeySet ks;
-    if (to_keyset(gks, ks)) return -1;
+    if (to_galois_keys(gks, ks)) return -1;
     std::vector<ExpandStep> sched = expand_schedule(&c, log_gap);
     for (ExpandStep& s : sched)
         if (lookup(&c, ks, level, s.galEl, s.key)) return -1;
@@ -462,7 +440,7 @@ int lgpu_ring_packing_pack(lgpu_ctx* ctx, int level, const uint64_t* cts_in, int
     PackPlan pl;
     if (pack_plan(&c, idx, n_cts, input_log_gap, zero_garbage_slots != 0, pl)) return -1;
     GaloisKeySet ks;
-    if (to_keyset(gks, ks)) return -1;
+    if (to_galois_keys(gks, ks)) return -1;
     for (u64 g : pl.galEl) {
         const GadgetCt* k = nullptr;
         if (lookup(&c, ks, level, g, k)) return -1;

@@ -103,11 +103,6 @@ namespace {
 
 constexpr unsigned kMaxGridZ = 65535;
 
-bool overlaps(const void* a, size_t abytes, const void* b, size_t bbytes) {
-    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-    return x < y + bbytes && y < x + abytes;
-}
-
 int log2_exact(int v) {
     int l = 0;
     while ((1 << l) < v) l++;
@@ -144,12 +139,7 @@ int apply_same(const Ctx* c, int level, bool ntt, const u64* in, size_t in_cs, u
         const size_t nq = level + 1, np = key.levelP + 1, qp = (nq + np) * N;
         Scratch acc_buf;
         if (acc_buf.alloc((size_t)2 * nb * qp, st)) return -1;
-        AccSpans acc;
-        for (int k = 0; k < 2; k++) {
-            u64* base = acc_buf.p + (size_t)k * nb * qp;
-            acc.q[k] = Span{base, N, qp};
-            acc.p[k] = Span{base + nq * N, N, qp};
-        }
+        const AccSpans acc = stacked_acc(acc_buf.p, nq, np, N, nb);
         if (gadget_product_lazy(c, level, CSpan{in + in_cs, N, 2 * in_cs}, key, acc, nb, st)) return -1;
         if (moddown_ntt_fused(c, level, key.levelP, acc_buf.p, 0, qp, in, 0, 2 * in_cs, out, 0, 2 * out_cs, 1, nb, st)) return -1;
         return moddown_ntt_fused(c, level, key.levelP, acc_buf.p + (size_t)nb * qp, 0, qp, nullptr, 0, 0, out + out_cs, 0, 2 * out_cs, 1, nb, st);
@@ -263,11 +253,8 @@ int lgpu_evaluator_apply_evaluation_key(lgpu_ctx* ctx, const uint64_t* ct_in, in
     const size_t in_b = (size_t)2 * (level_in + 1) * n_in * 8 * batch, out_b = (size_t)2 * (level_out + 1) * n_out * 8 * batch;
     if (!(n_in == n_out && ct_in == ct_out && level_in == level_out))
         REQUIRE(!overlaps(ct_in, in_b, ct_out, out_b), "ct_out overlaps ct_in (only ct_out == ct_in at the same degree and level is allowed)");
-    REQUIRE(evk && evk->data, "null evaluation key");
-    REQUIRE_ALIGNED(AL(evk->data));
     GadgetCt key;
-    key.data = (const u64*)evk->data; key.levelQ = evk->level_q; key.levelP = evk->level_p; key.pw2 = evk->base_two_decomposition;
-    key.ndigits = evk->n_digits; key.npw2max = evk->n_pw2_max > 0 ? evk->n_pw2_max : 1; key.pw2_sizes = evk->pw2_sizes;
+    if (to_gadget_ct(evk, key)) return -1;
     const int level = std::min(level_in, level_out);
     if (check_evk(&c, level, key)) return -1;
     REQUIRE(key.levelP <= 0 || key.pw2 == 0, "BaseTwoDecomposition != 0 requires levelP <= 0");

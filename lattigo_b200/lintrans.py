@@ -34,11 +34,8 @@ class Evaluator:
 
     def __init__(self, ctx: Context, galois_keys: Dict[int, GadgetCiphertext]):
         self.ctx = ctx
-        self.keys = dict(galois_keys)
-        els = list(self.keys.keys())
-        self._els = (ctypes.c_uint64 * max(1, len(els)))(*els)
-        self._structs = (_lib.GadgetCtStruct * max(1, len(els)))(*[self.keys[g].struct for g in els])
-        self._gks = _lib.GaloisKeysStruct(len(els), self._els, self._structs)
+        keys = _lib.GaloisKeys(galois_keys)
+        self.keys, self._gks = keys.keys, keys.gks
 
     def GaloisElement(self, k: int) -> int:
         return int(_lib.lib().lgpu_galois_element(self.ctx.h, k))

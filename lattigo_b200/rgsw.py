@@ -34,17 +34,13 @@ class BlindRotationEvaluator:
     (eprint 2022/198), driven by the host-side LWE mask `a` (values modulo 2N), in place on `acc` ((2, level+1, N), NTT domain)."""
 
     def __init__(self, ctx: Context, blind_rotation_keys, automorphism_keys, window_size: int = 10):
-        import ctypes
         self.ctx = ctx
         self.brk = list(blind_rotation_keys)                      # rgsw.Ciphertext per LWE coefficient: RGSW(X^{s_j})
         n = len(self.brk)
         self._b0 = (_lib.GadgetCtStruct * n)(*[k.Value[0].struct for k in self.brk])
         self._b1 = (_lib.GadgetCtStruct * n)(*[k.Value[1].struct for k in self.brk])
-        self.keys = dict(automorphism_keys)                       # {galEl: GadgetCiphertext}
-        els = list(self.keys.keys())
-        self._els = (ctypes.c_uint64 * max(1, len(els)))(*els)
-        self._structs = (_lib.GadgetCtStruct * max(1, len(els)))(*[self.keys[g].struct for g in els])
-        self._gks = _lib.GaloisKeysStruct(len(els), self._els, self._structs)
+        keys = _lib.GaloisKeys(automorphism_keys)                 # {galEl: GadgetCiphertext}
+        self.keys, self._gks = keys.keys, keys.gks
         self.window = window_size
 
     def BlindRotateCore(self, a, acc):

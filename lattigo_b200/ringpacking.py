@@ -53,26 +53,14 @@ def getMinimumGap(keys: List[int]) -> Tuple[int, int]:
     return gap, logGap
 
 
-class _Keys:
-    """The lgpu_galois_keys view of {galEl: GadgetCiphertext}. The structs point into the keys' device tensors and host arrays, so
-    the view holds the keys themselves for as long as it lives."""
-
-    def __init__(self, keys: Dict[int, GadgetCiphertext]):
-        self.keys = dict(keys)
-        els = list(self.keys)
-        self._els = (ctypes.c_uint64 * max(1, len(els)))(*els)
-        self._structs = (_lib.GadgetCtStruct * max(1, len(els)))(*[self.keys[g].struct for g in els])
-        self.gks = _lib.GaloisKeysStruct(len(els), self._els, self._structs)
-
-
 class RingPackingEvaluator:
     """rlwe.RingPackingEvaluator with MinLogN == MaxLogN == ctx.logN. extract_keys / repack_keys: {galEl: GadgetCiphertext}
     (RingPackingEvaluationKey.ExtractKeys / RepackKeys at that degree; see GaloisElementsForExpand / GaloisElementsForPack)."""
 
     def __init__(self, ctx: Context, extract_keys: Dict[int, GadgetCiphertext], repack_keys: Dict[int, GadgetCiphertext]):
         self.ctx = ctx
-        self._extract = _Keys(extract_keys)
-        self._repack = _Keys(repack_keys)
+        self._extract = _lib.GaloisKeys(extract_keys)
+        self._repack = _lib.GaloisKeys(repack_keys)
 
     def Expand(self, ct, logGap: int, is_ntt: bool = True) -> Dict[int, object]:
         """:457-571. Returns {j: ciphertext} for the N / 2^logGap multiples j of 2^logGap, each encrypting coefficient j of ct at
