@@ -790,6 +790,11 @@ int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_r
         if (accb.alloc((size_t)2 * batch * (nq + np) * N, st)) return -1;
         const AccSpans acc = stacked_acc(accb.p, nq, np, N, batch);
         if (gadget_product_lazy(c, level, CSpan{d2, N, nq * N}, rlk, acc, batch, st)) return -1;
+        if (nb_rescales == 1 && moddown_rescale_applicable(c, level)) {
+            const size_t nqo = nq - 1;
+            return moddown_rescale_ntt_fused(c, level, rlk.levelP, accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N, d0, (size_t)batch * nq * N,
+                                             nq * N, out, nqo * N, 2 * nqo * N, 2, batch, st);
+        }
         // d0, d1 are consecutive [comp][batch][nq][N] blocks: out = d + ModDown(acc), in place
         if (moddown_ntt_fused(c, level, rlk.levelP, accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N, d0, (size_t)batch * nq * N, nq * N,
                               d0, (size_t)batch * nq * N, nq * N, 2, batch, st)) return -1;

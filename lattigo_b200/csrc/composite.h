@@ -101,6 +101,10 @@ int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size
                       u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st);
 int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs,
                              int ncomp, int batch, cudaStream_t st);
+// moddown_ntt_fused with addend D followed by div_round_last_ntt_fused (D is overwritten), in fewer passes when Q[levelQ] is an FP64-pipe prime
+bool moddown_rescale_applicable(const Ctx* c, int level);
+int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, u64* D, size_t d_cs,
+                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st);
 
 int ckks_mulrelin_rescale(const Ctx* c, int level, const u64* ctA, const u64* ctB, const GadgetCt& rlk, int nb_rescales, u64* out, int batch,
                           cudaStream_t st);

@@ -61,6 +61,11 @@ static int k2_split() {
     static const int v = [] { const char* e = getenv("LGPU_K2_SPLIT"); return e ? atoi(e) : 1; }();
     return v;
 }
+// LGPU_K2_J4=0: every K2 launch takes the plain kernel (ks_strided_kernel) instead of the row-sharing one (ks_strided_j4_kernel)
+static int k2_j4() {
+    static const int v = [] { const char* e = getenv("LGPU_K2_J4"); return e ? atoi(e) : 1; }();
+    return v;
+}
 static int k2_fpsum() {
     static const int on = [] { const char* e = getenv("LGPU_K2_FPSUM"); return e && atoi(e) ? 1 : 0; }();
     return on;
@@ -145,6 +150,7 @@ struct KsStridedParams {
     // PRO_BCAST (rescale): e = cred(bc[x] + bc_add, bc_q) + s0[launch row]
     const u64* bc; size_t bc_bs; u64 bc_add, bc_q;
     u64 s0[kMaxRows];
+    double bc_mul[kMaxRows];        // ModDown fused with the rescale: [P]_q of the launch row (ks_add_bcast)
     KsDigit dg[kMaxDigits];
 };
 
@@ -191,6 +197,21 @@ __device__ __forceinline__ double ks_ext_split(const u64 (&y)[NSMAX], const u32 
     const double bb = __longlong_as_double((long long)(B | 0x4330000000000000ull));                 // 2^52 + B
     const double t = fp_reduce(__fma_rn(bb, 8388608.0, -37778931862957161709568.0), fq, fqinv);     // (2^52 + B) 2^23 - 2^75 = B 2^23, exact
     return fp_reduce(__dadd_rn(__dadd_rn(ab, vtb), t), fq, fqinv);                                  // (2^52 + A) + (vt - half_t - 2^52), exact
+}
+
+// The ModDown fused with the rescale by q_L that follows it (moddown_rescale_ntt_fused), on FP64 target rows with an FP64-pipe q_L:
+// to the extension m of the ModDown (an integer in [0, 3q) from ks_ext, or a double in (-0.66q, 0.66q) from ks_ext_split) this adds
+// [P]_q e, where e = cred(bc + bc_add, q_L) + s0 < q_L + q is the rescale's value of PRO_BCAST. Both q and q_L are fp_ok
+// ((10 + logN) q < 2^51, logN >= 13), so e < 2^47.5 is exact as a double, |e [P]_q / q| 2^-53 < 2^-5 keeps the quotient of fp_mulmod
+// off by at most one and its rounding error below 2^-5 q, and |fp_mulmod(e, [P]_q)| < 0.57q. The sum lies in (-2q, 4q): inside the
+// |x| < 10q that the forward FP64 transform takes (each of its logN stages adds less than q, and (10 + logN) q < 2^51).
+template <int R>
+__device__ __forceinline__ void ks_add_bcast(double (&x)[R], const KsStridedParams& p, int b, int jrow, int l, double fq, double fqinv) {
+    const u64* bc = p.bc + (size_t)b * p.bc_bs + l;
+    const u64 s0 = p.s0[jrow];
+    const double pm = p.bc_mul[jrow];
+#pragma unroll
+    for (int k = 0; k < R; k++) x[k] = __dadd_rn(x[k], fp_mulmod(u2d(cred(bc[k * 4096] + p.bc_add, p.bc_q) + s0), pm, fq, fqinv));
 }
 
 enum { PRO_MODUP = 0, PRO_BCAST = 1 };
@@ -362,9 +383,11 @@ __global__ void __launch_bounds__(256, KS_STRIDED_MINB) ks_strided_kernel(KsStri
 // Here a CTA owns 64 strided columns (l) x all R strided coefficients and stages that y/v tile in shared memory once
 // for J = 4 target rows (thread = (column, target row)): L2 traffic drops 4x, the y reads become conflict-free /
 // broadcast shared-memory loads. Multi-source digits only (the single-limb rule keeps the plain kernel).
+// BC (FP64 rows only): the ModDown's extension plus the rescale's broadcast term, see ks_add_bcast.
 // ------------------------------------------------------------------------------------------------------------
-template <int RL, int NSMAX, bool FP, bool CORR = true>
+template <int RL, int NSMAX, bool FP, bool CORR = true, bool BC = false>
 __global__ void __launch_bounds__(256, KS_STRIDED_J4_MINB) ks_strided_j4_kernel(KsStridedParams p) {
+    static_assert(FP || !BC, "the fused rescale term is added on FP64 rows only");
     constexpr int R = 1 << RL, J = KS_J, LB = 256 / J;
     extern __shared__ u64 dsm[];
     u64* s_y = dsm;                                                        // [NSMAX][R][LB]
@@ -443,6 +466,7 @@ __global__ void __launch_bounds__(256, KS_STRIDED_J4_MINB) ks_strided_j4_kernel(
                 for (int i = 0; i < NSMAX; i++) y[i] = s_y[(i * R + k) * LB + lx];
                 x[k] = ks_ext_split<NSMAX>(y, c0, c1, d0, d1, s_vtd[jj][s_v[k * LB + lx]], fq, fqinv);
             }
+            if constexpr (BC) ks_add_bcast<R>(x, p, b, jrow, l, fq, fqinv);
 #pragma unroll
             for (int u = 0; u < RL; u++) {
                 const int half = 1 << (RL - 1 - u);
@@ -480,6 +504,7 @@ __global__ void __launch_bounds__(256, KS_STRIDED_J4_MINB) ks_strided_j4_kernel(
         double x[R];
 #pragma unroll
         for (int k = 0; k < R; k++) x[k] = u2d(e[k]);
+        if constexpr (BC) ks_add_bcast<R>(x, p, b, jrow, l, fq, fqinv);
 #pragma unroll
         for (int u = 0; u < RL; u++) {
             const int half = 1 << (RL - 1 - u);
@@ -1013,23 +1038,31 @@ bool ks_fused_applicable(const Ctx* c, int levelQ, const GadgetCt& evk) {
     return true;
 }
 
-template <int RL, int NSMAX, bool FP, bool CORR>
+template <int RL, int NSMAX, bool FP, bool CORR, bool BC = false>
 static int ks_launch_j4(const KsStridedParams& p, dim3 grid, cudaStream_t st) {
     constexpr int R = 1 << RL;
     constexpr int LB = 256 / KS_J;
     const size_t smem = (size_t)NSMAX * R * LB * sizeof(u64) + (size_t)R * LB;
-    LGPU_CUDA_OK(cudaFuncSetAttribute(ks_strided_j4_kernel<RL, NSMAX, FP, CORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ks_strided_j4_kernel<RL, NSMAX, FP, CORR><<<dim3(grid.x * KS_J, (grid.y + KS_J - 1) / KS_J, grid.z), 256, smem, st>>>(p);
+    LGPU_CUDA_OK(cudaFuncSetAttribute(ks_strided_j4_kernel<RL, NSMAX, FP, CORR, BC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ks_strided_j4_kernel<RL, NSMAX, FP, CORR, BC><<<dim3(grid.x * KS_J, (grid.y + KS_J - 1) / KS_J, grid.z), 256, smem, st>>>(p);
     LGPU_CUDA_OK(cudaGetLastError());
     return 0;
+}
+
+// K2 of the ModDown fused with the rescale (FP64 rows, row-sharing kernel only: 2^13 <= N <= 2^16)
+static int ks_launch_moddown_bcast(int rl, int nsmax, const KsStridedParams& p, dim3 grid, cudaStream_t st) {
+#define KS_MB(RLV) case RLV: return nsmax <= 4 ? ks_launch_j4<RLV, 4, true, true, true>(p, grid, st) : ks_launch_j4<RLV, 8, true, true, true>(p, grid, st);
+    switch (rl) { KS_MB(1) KS_MB(2) KS_MB(3) KS_MB(4) default: break; }
+#undef KS_MB
+    set_error("unsupported strided radix");
+    return -1;
 }
 
 // CORR: the integer rows of the launch need the lazy-correction schedule (some prime above 2^57); ignored for FP64 rows
 template <bool FP, int PRO = PRO_MODUP, bool CORR = true>
 static int ks_launch_strided(int rl, int nsmax, const KsStridedParams& p, dim3 grid, cudaStream_t st) {
     if constexpr (PRO == PRO_MODUP) {
-        static const int j4 = [] { const char* e = getenv("LGPU_K2_J4"); return e ? atoi(e) : 1; }();
-        bool multi = j4 != 0 && rl <= 4;                       // R = 32 (N = 2^17) would need 2 x 66 KB of shared memory
+        bool multi = k2_j4() != 0 && rl <= 4;                      // R = 32 (N = 2^17) would need 2 x 66 KB of shared memory
         for (int d = 0; d < p.nd; d++) multi = multi && (p.dg[d].nS > 1 || !p.single_rule);
         if (multi) {
 #define KS_J4(RLV) case RLV: return nsmax <= 4 ? ks_launch_j4<RLV, 4, FP, CORR>(p, grid, st) : ks_launch_j4<RLV, 8, FP, CORR>(p, grid, st);
@@ -1213,7 +1246,9 @@ struct FzChunkParams {
     const u64* D; size_t d_cs, d_bs;
     u64* out; size_t o_cs, o_bs;
     int nb, logN;
+    int dscale;         // 1: the addend is scaled, out = CRed(MRed(x + 2q - a, s) + MRed(d, s2)) (ModDown fused with the rescale)
     u64 s[kMaxRows];
+    u64 s2[kMaxRows];
 };
 
 template <bool FP>
@@ -1277,7 +1312,7 @@ __global__ void __launch_bounds__(256, 2) fz_chunk_epi_kernel(FzChunkParams p) {
                 x = x >= L.kq ? x - L.kq : x;
             }
             u64 r = mred(x + twoq - a[j], sc, q, qinv);
-            if (D) r = cred(r + d[j], q);
+            if (D) r = cred(r + (p.dscale ? mred(d[j], p.s2[blockIdx.y], q, qinv) : d[j]), q);
             out[idx] = r;
         }
     }
@@ -1344,6 +1379,10 @@ __global__ void __launch_bounds__(512, 2) fz_chunk_epi_fp8_kernel(FzChunkParams 
         const u64 xb = KS_LAZY_X ? fp_biased_u64(x[2 * j + 1], off52) : fp_canon(x[2 * j + 1], fq, fqinv);
         r[j].x = mred(xa + twoq - a[j].x, sc, q, qinv);
         r[j].y = mred(xb + twoq - a[j].y, sc, q, qinv);
+        if (D && p.dscale) {
+            const u64 sc2 = p.s2[blockIdx.y];
+            d[j].x = mred(d[j].x, sc2, q, qinv); d[j].y = mred(d[j].y, sc2, q, qinv);
+        }
         if (D) { r[j].x = cred(r[j].x + d[j].x, q); r[j].y = cred(r[j].y + d[j].y, q); }
     }
 #pragma unroll
@@ -1446,16 +1485,22 @@ bool fz_applicable(const Ctx* c, int levelQ, int levelP) {
 // Fused Evaluator.ModDown (NTT -> NTT, core/rlwe/evaluator_gadget_product.go:39-52 = 2 x ModDownQPtoQNTT,
 // ring/basis_extension.go:235-256) for ncomp x batch QP-stacked accumulators, with an optional addend:
 //     out[c][b] = (accQ[c][b] - NTT(ModUpPtoQ(INTT(accP[c][b])))) * P^-1  (+ D[c][b])
-int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs, size_t d_bs,
-                      u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st) {
+// Scratch: buffP and Y [Z][np][N], P1 [Z][nq][N], V [Z][N] bytes.
+static size_t moddown_scratch_words(int nq, int np, int Z, size_t N) { return 2 * (size_t)Z * np * N + (size_t)Z * nq * N + ((size_t)Z * N + 7) / 8; }
+
+// the K1 outputs of the fused ModDown and the K2 / epilogue parameters of its target rows
+struct FzModDown {
+    KsStridedParams sp;
+    FzChunkParams cp;
+};
+
+// A (INTT of the P rows) and B (K1) of the fused ModDown; fills md for fz_moddown_rows
+static int fz_moddown_prepare(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs,
+                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, u64* buf, FzModDown& md, cudaStream_t st) {
     const int nq = levelQ + 1, np = levelP + 1;
     const size_t N = c->N;
     const int Z = ncomp * batch;
-    const int s1 = c->logN - 12;
-    const size_t bp_words = (size_t)Z * np * N, y_words = bp_words, p1_words = (size_t)Z * nq * N, v_words = ((size_t)Z * N + 7) / 8;
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, (bp_words + y_words + p1_words + v_words) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    const size_t bp_words = (size_t)Z * np * N, y_words = bp_words, p1_words = (size_t)Z * nq * N;
     u64* buffP = buf; u64* Y = buffP + bp_words; u64* P1 = Y + y_words;
     unsigned char* V = reinterpret_cast<unsigned char*>(P1 + p1_words);
     // A: INTT of the P rows
@@ -1481,9 +1526,7 @@ int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size
         LGPU_CUDA_OK(cudaGetLastError());
     }
     // C: basis extension folded into the strided pass
-    RowMap fp, in;
-    split_rows(c, 0, nq, fp, in);
-    KsStridedParams sp;
+    KsStridedParams& sp = md.sp;
     memset(&sp, 0, sizeof(sp));
     sp.limbs = c->d_limbs; sp.blob = c->d_blob; sp.Y = Y; sp.y_bs = (size_t)np * N; sp.V = V; sp.v_bs = N;
     sp.P1 = P1; sp.p1_ds = (size_t)nq * N; sp.p1_bs = (size_t)nq * N;
@@ -1496,15 +1539,26 @@ int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size
         for (int j = 0; j < np; j++) fps = fps && c->h_limbs[c->nQ + j].fp_ok;
         sp.dg[0].fp_src = fps ? (unsigned short)(1 + k2_fpsum()) : 0;
     }
-    FzChunkParams cp;
+    FzChunkParams& cp = md.cp;
     memset(&cp, 0, sizeof(cp));
     cp.limbs = c->d_limbs; cp.P1 = P1; cp.p1_bs = (size_t)nq * N;
     cp.A = acc; cp.a_cs = acc_cs; cp.a_bs = acc_bs; cp.D = D; cp.d_cs = d_cs; cp.d_bs = d_bs;
     cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.nb = batch; cp.logN = c->logN;
+    return 0;
+}
+
+// C of the fused ModDown on the target rows fp (FP64 class, stream st) and in (integer classes, stream sint)
+static int fz_moddown_rows(const Ctx* c, int levelP, FzModDown& m, const RowMap& fp, const RowMap& in, int ncomp, int batch, cudaStream_t st,
+                           cudaStream_t sint) {
+    KsStridedParams& sp = m.sp;
+    FzChunkParams& cp = m.cp;
+    const size_t N = c->N;
+    const int Z = ncomp * batch, np = levelP + 1;
+    const int s1 = c->logN - 12;
+    const bool D = cp.D != nullptr;
     const unsigned gx = (unsigned)(((N >> s1) + 255) / 256);
     const unsigned chunks = (unsigned)(N >> 12);
     auto scal = [&](const RowMap& rm) { for (int r = 0; r < rm.nrows; r++) { const int i = rm.drow[r]; cp.s[r] = c->Q[i] - c->mdc_PtoQ[(size_t)levelP * c->nQ + i]; } };
-    cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
     RowMap in_c, in_n;
     split_by_corr(c, in, in_c, in_n);
     for (int pass = 0; pass < 2; pass++) {
@@ -1524,21 +1578,36 @@ int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size
         ProfScope ps(LGPU_KCLASS_EPILOGUE, st, 8.0 * N * Z * fp.nrows * ((D ? 5.0 : 4.0) - 1.0), 1);
         cp.rm = fp; scal(fp); if (fz_launch_chunk<true>(cp, dim3(chunks, fp.nrows, Z), st)) return -1;
     }
+    return 0;
+}
+
+int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs, size_t d_bs,
+                      u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st) {
+    const int nq = levelQ + 1;
+    u64* buf = nullptr;
+    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, moddown_scratch_words(nq, levelP + 1, ncomp * batch, c->N) * sizeof(u64), st));
+    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    FzModDown m;
+    if (fz_moddown_prepare(c, levelQ, levelP, acc, acc_cs, acc_bs, D, d_cs, d_bs, out, o_cs, o_bs, ncomp, batch, buf, m, st)) return -1;
+    RowMap fp, in;
+    split_rows(c, 0, nq, fp, in);
+    cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
+    if (fz_moddown_rows(c, levelP, m, fp, in, ncomp, batch, st, sint)) return -1;
     join_side(c, st, sint);
     return 0;
 }
 
 // Fused Ring.DivRoundByLastModulusNTT (ring/scaling.go:101-122) for ncomp x batch polynomials at level `level`:
 // X rows 0..level -> out rows 0..level-1.
-int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs,
-                             int ncomp, int batch, cudaStream_t st) {
+struct FzRescale {
+    KsStridedParams sp;
+    FzChunkParams cp;
+};
+
+// the INTT r [ncomp][batch][N] of row `level` of X, and the K2 / epilogue parameters of the rescale (P1: [Z] x p1_bs words)
+static int fz_rescale_prepare(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp,
+                              int batch, u64* r, u64* P1, size_t p1_bs, FzRescale& m, cudaStream_t st) {
     const size_t N = c->N;
-    const int Z = ncomp * batch;
-    const int s1 = c->logN - 12;
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, ((size_t)Z * N + (size_t)Z * level * N) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
-    u64* r = buf; u64* P1 = buf + (size_t)Z * N;
     RowMap rl;
     rl.nrows = 1; rl.limb[0] = (unsigned char)level; rl.drow[0] = 0;
     for (int cc = 0; cc < ncomp; cc++) {
@@ -1546,25 +1615,32 @@ int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs,
         Span o{r + (size_t)cc * batch * N, N, N};
         if (launch_intt(c, rl, in, o, batch, NTT_CANONICAL, st)) return -1;
     }
-    const u64 qL = c->Q[level];
-    const u64 pHalf = (qL - 1) >> 1;
-    RowMap fp, in;
-    split_rows(c, 0, level, fp, in);
-    KsStridedParams sp;
+    KsStridedParams& sp = m.sp;
     memset(&sp, 0, sizeof(sp));
-    sp.limbs = c->d_limbs; sp.blob = c->d_blob; sp.P1 = P1; sp.p1_ds = (size_t)level * N; sp.p1_bs = (size_t)level * N;
+    sp.limbs = c->d_limbs; sp.blob = c->d_blob; sp.P1 = P1; sp.p1_ds = p1_bs; sp.p1_bs = p1_bs;
     sp.logN = c->logN; sp.nq = level; sp.k = 1; sp.nd = 1;
-    sp.bc = r; sp.bc_bs = N; sp.bc_add = pHalf; sp.bc_q = qL;
-    FzChunkParams cp;
+    sp.bc = r; sp.bc_bs = N; sp.bc_add = (c->Q[level] - 1) >> 1; sp.bc_q = c->Q[level];
+    FzChunkParams& cp = m.cp;
     memset(&cp, 0, sizeof(cp));
-    cp.limbs = c->d_limbs; cp.P1 = P1; cp.p1_bs = (size_t)level * N;
+    cp.limbs = c->d_limbs; cp.P1 = P1; cp.p1_bs = p1_bs;
     cp.A = X; cp.a_cs = x_cs; cp.a_bs = x_bs; cp.D = nullptr;
     cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.nb = batch; cp.logN = c->logN;
+    return 0;
+}
+
+// K2 (PRO_BCAST) and epilogue of the rescale on the rows fp (FP64 class, stream st) and in (integer classes, stream sint)
+static int fz_rescale_rows(const Ctx* c, int level, FzRescale& m, const RowMap& fp, const RowMap& in, int ncomp, int batch, cudaStream_t st,
+                           cudaStream_t sint) {
+    KsStridedParams& sp = m.sp;
+    FzChunkParams& cp = m.cp;
+    const size_t N = c->N;
+    const int Z = ncomp * batch;
+    const int s1 = c->logN - 12;
+    const u64 pHalf = sp.bc_add;
     const unsigned gx = (unsigned)(((N >> s1) + 255) / 256);
     const unsigned chunks = (unsigned)(N >> 12);
     auto s0 = [&](const RowMap& rm) { for (int k = 0; k < rm.nrows; k++) { const u64 qi = c->Q[rm.drow[k]]; sp.s0[k] = qi - (pHalf % qi); } };
     auto scal = [&](const RowMap& rm) { for (int k = 0; k < rm.nrows; k++) cp.s[k] = c->rescaleQ[(size_t)(level - 1) * c->nQ + rm.drow[k]]; };
-    cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
     RowMap in_c, in_n;
     split_by_corr(c, in, in_c, in_n);
     for (int pass = 0; pass < 2; pass++) {
@@ -1583,6 +1659,90 @@ int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs,
           sp.rm = fp; s0(fp); if (ks_launch_strided<true, PRO_BCAST>(s1, 1, sp, dim3(gx, fp.nrows, Z), st)) return -1; }
         ProfScope ps(LGPU_KCLASS_EPILOGUE, st, 8.0 * N * Z * fp.nrows * (4.0 - 1.0), 1);
         cp.rm = fp; scal(fp); if (fz_launch_chunk<true>(cp, dim3(chunks, fp.nrows, Z), st)) return -1;
+    }
+    return 0;
+}
+
+int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs,
+                             int ncomp, int batch, cudaStream_t st) {
+    const size_t N = c->N;
+    const int Z = ncomp * batch;
+    u64* buf = nullptr;
+    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, ((size_t)Z * N + (size_t)Z * level * N) * sizeof(u64), st));
+    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    FzRescale m;
+    if (fz_rescale_prepare(c, level, X, x_cs, x_bs, out, o_cs, o_bs, ncomp, batch, buf, buf + (size_t)Z * N, (size_t)level * N, m, st)) return -1;
+    RowMap fp, in;
+    split_rows(c, 0, level, fp, in);
+    cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
+    if (fz_rescale_rows(c, level, m, fp, in, ncomp, batch, st, sint)) return -1;
+    join_side(c, st, sint);
+    return 0;
+}
+
+// LGPU_FUSED_RESCALE (default 1; 0 = moddown_ntt_fused, then div_round_last_ntt_fused): moddown_rescale_ntt_fused. Its merged K2 exists in the
+// row-sharing kernel only, so LGPU_K2_J4=0 selects the two stages too.
+bool moddown_rescale_applicable(const Ctx* c, int level) {
+    static const int on = [] { const char* e = getenv("LGPU_FUSED_RESCALE"); return e ? atoi(e) : 1; }();
+    return on && k2_j4() && level >= 1 && c->h_limbs[level].fp_ok && fp64_ntt_supported(c);
+}
+
+// ModDown with an addend, then the rescale by q_L = Q[levelQ], for ncomp x batch QP-stacked accumulators, when q_L is an FP64-pipe prime:
+//     out[c][b] = DivRoundByLastModulusNTT(ModDown(acc[c][b]) + D[c][b])          (moddown_ntt_fused, then div_round_last_ntt_fused)
+// Row L and the integer rows take the two stages (the ModDown's result X goes to D in place, as the rescale reads it). On the FP64 rows
+// i < L they are one K2 and one epilogue pass, which read acc and D and write out: the NTT is linear mod q_i, hence
+//     out_i = (X_i - NTT(e_i)) q_L^-1 = (acc_i - NTT(m_i + [P]_{q_i} e_i)) (P q_L)^-1 + D_i q_L^-1,
+// with m_i the ModDown's basis extension and e_i the rescale's broadcast value of INTT(X_L), both computed as in the two stages: the
+// canonical outputs are the same. D keeps its FP64 rows below L.
+int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, u64* D, size_t d_cs,
+                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st) {
+    const int nq = levelQ + 1, np = levelP + 1, L = levelQ;
+    const size_t N = c->N;
+    const int Z = ncomp * batch;
+    const int s1 = c->logN - 12;
+    const size_t md_words = moddown_scratch_words(nq, np, Z, N);
+    u64* buf = nullptr;
+    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, (md_words + (size_t)Z * N) * sizeof(u64), st));
+    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    u64* r = buf + md_words;
+    FzModDown md;
+    if (fz_moddown_prepare(c, levelQ, levelP, acc, acc_cs, acc_bs, D, d_cs, d_bs, D, d_cs, d_bs, ncomp, batch, buf, md, st)) return -1;
+    RowMap fp, in, last, none;
+    split_rows(c, 0, L, fp, in);
+    last.nrows = 1; last.limb[0] = last.drow[0] = (unsigned char)L;
+    none.nrows = 0;
+    // the ModDown on row L and the integer rows
+    cudaStream_t sint = fork_side(c, st, in.nrows > 0);
+    if (fz_moddown_rows(c, levelP, md, last, in, ncomp, batch, st, sint)) return -1;
+    join_side(c, st, sint);
+    // INTT of X_L; the rescale of the integer rows (the ModDown's P1 rows are free again)
+    FzRescale rs;
+    if (fz_rescale_prepare(c, L, D, d_cs, d_bs, out, o_cs, o_bs, ncomp, batch, r, md.sp.P1, (size_t)nq * N, rs, st)) return -1;
+    sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
+    if (fz_rescale_rows(c, L, rs, none, in, ncomp, batch, st, sint)) return -1;
+    // the FP64 rows below L: one K2 and one epilogue
+    if (fp.nrows) {
+        KsStridedParams& sp = md.sp;
+        sp.rm = fp; sp.bc = r; sp.bc_bs = N; sp.bc_add = rs.sp.bc_add; sp.bc_q = rs.sp.bc_q;
+        FzChunkParams cp = md.cp;
+        cp.rm = fp; cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.dscale = 1;
+        const u64 qL = c->Q[L];
+        for (int k = 0; k < fp.nrows; k++) {
+            const u64 qi = c->Q[fp.drow[k]];
+            u64 pm = 1;
+            for (int j = 0; j < np; j++) pm = h_mulmod(pm, c->P[j] % qi, qi);
+            const u64 qLinv = h_invmod(qL % qi, qi);
+            sp.s0[k] = qi - (sp.bc_add % qi);
+            sp.bc_mul[k] = (double)pm;
+            cp.s[k] = h_mform(qi - h_mulmod(h_invmod(pm, qi), qLinv, qi), qi);    // -(P q_L)^-1, Montgomery form
+            cp.s2[k] = h_mform(qLinv, qi);
+        }
+        {
+            ProfScope ps(LGPU_KCLASS_FUSED, st, 8.0 * N * Z * (fp.nrows + 1.0), 1);
+            if (ks_launch_moddown_bcast(s1, np, sp, dim3((unsigned)(((N >> s1) + 255) / 256), fp.nrows, Z), st)) return -1;
+        }
+        ProfScope ps(LGPU_KCLASS_EPILOGUE, st, 8.0 * N * Z * fp.nrows * 4.0, 1);
+        if (fz_launch_chunk<true>(cp, dim3((unsigned)(N >> 12), fp.nrows, Z), st)) return -1;
     }
     join_side(c, st, sint);
     return 0;
