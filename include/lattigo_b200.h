@@ -581,6 +581,40 @@ int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const
                             int scale_invariant, int nb_rescales, uint64_t* ct_out, int batch, void* stream);
 
 
+/* ---- BGV / BFV encoder (schemes/bgv/encoder.go; BFV uses the same bgv.Encoder) ---------------------------------------
+ * lgpu_bgv_encoder_create: the plaintext ring T of bgv.NewParameters (params.go:76-135) and the tables of NewEncoder (encoder.go:49-133)
+ * for ctx's Q and plaintext modulus t. Checks, in the reference's terms: t >= 2, t < Q[0], t not in Q, `order` (the largest power of
+ * two with t = 1 mod order) >= 16, t prime with t = 1 mod 2n for n = min(N, order / 2). One deliberate difference: n < 16 (t = 1 mod 16
+ * but not mod 32, e.g. t = 17) is rejected, since the engine's transforms start at 16 points. Standard ring only. A host-only ctx gives
+ * a host-only handle (argument checks, no device execution). Independent of lgpu_bgv; destroy before ctx.
+ *
+ * flags: LGPU_ENC_NTT = MetaData.IsNTT, LGPU_ENC_MONTGOMERY = MetaData.IsMontgomery (ignored by the coefficient Encode and by Decode, as in
+ * the reference), LGPU_ENC_COEFFS = IsBatched false, LGPU_ENC_SIGNED: the values are int64 rather than uint64, LGPU_ENC_SCALE_UP:
+ * multiply by t^-1 mod Q (Encode; without it the call is Embed). scale = MetaData.Scale.Uint64(), any value. `values` are device arrays
+ * of 64-bit words; strides are in words; batch <= 65535. Every check runs before any launch, also on a host-only handle; inputs are never
+ * written; scratch is stream-ordered (cudaMallocAsync on `stream`).
+ *
+ * Encode: EncodeRingT + EmbedScale (encoder.go:201-333) of n_values <= n (MaxSlots) values per entry, the unmapped slots zero, into out_q
+ * (level_q + 1 rows) and, for Embed only (no LGPU_ENC_SCALE_UP), out_p (level_p + 1 rows of a ringqp.Poly; level_p = -1: none). Words
+ * are canonical, except that Embed without NTT or Montgomery keeps the reference's literal ring-T word on a row whose q_i < t. With
+ * LGPU_ENC_COEFFS (Encode with IsBatched false, encoder.go:148-199; LGPU_ENC_SCALE_UP required, level_p = -1): n_values <= N words as
+ * coefficients, uint64 words unreduced, MulScalar(scale) mod t, RingT2Q(scaleUp), NTT when LGPU_ENC_NTT.
+ *
+ * Decode: Decode (encoder.go:471-521) of `batch` plaintexts pt [level + 1][N] (INTT first when LGPU_ENC_NTT; coefficient-domain words may
+ * be any 64-bit value): RingQ2T(scaleDown), then MulScalar(scale^-1 mod t); batched: ring-T NTT and the n slots into `values`; with
+ * LGPU_ENC_COEFFS: uint64 gives N words, int64 (LGPU_ENC_SIGNED) centres only the first n words and leaves the rest of the entry
+ * untouched, as the reference does. Signed words are v - t for v >= t >> 1. Q_level up to 4096 bits. */
+#define LGPU_ENC_SIGNED 8
+#define LGPU_ENC_SCALE_UP 16
+typedef struct lgpu_bgv_encoder lgpu_bgv_encoder;
+int lgpu_bgv_encoder_create(lgpu_ctx* ctx, uint64_t t, lgpu_bgv_encoder** out);
+void lgpu_bgv_encoder_destroy(lgpu_bgv_encoder* enc);
+int lgpu_bgv_encode(lgpu_bgv_encoder* enc, const uint64_t* values, int n_values, int flags, uint64_t scale, int level_q, uint64_t* out_q,
+                    int level_p, uint64_t* out_p, int batch, size_t values_stride, size_t out_q_stride, size_t out_p_stride, void* stream);
+int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int level, int flags, uint64_t scale, uint64_t* values, int batch,
+                    size_t pt_stride, size_t values_stride, void* stream);
+
+
 /* ---- launch accounting / profiling (used by bench.py) ------------------------------------------------------- */
 enum lgpu_kclass {
     LGPU_KCLASS_NTT_FWD = 0,   /* one forward transform of rows x batch polynomials (1 or 2 kernels) */

@@ -16,3 +16,4 @@ from . import rgsw  # noqa: F401,E402
 from . import encryptor  # noqa: F401,E402
 from . import ckks_fft  # noqa: F401,E402
 from .encoder import Encoder  # noqa: F401,E402
+from .bgv_encoder import BGVEncoder  # noqa: F401,E402

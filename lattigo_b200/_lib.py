@@ -104,6 +104,10 @@ def lib():
             "lgpu_ckks_special_fft": [vp, vp, i, i, vp, vp, i, i, z, vp],
             "lgpu_ckks_encode": [vp, vp, i, i, c.c_double, i, vp, vp, i, vp, i, vp, i, z, z, z, vp],
             "lgpu_ckks_decode": [vp, vp, i, i, c.c_double, i, c.c_double, vp, vp, vp, i, z, z, vp],
+            "lgpu_bgv_encoder_create": [vp, u64, c.POINTER(vp)],
+            "lgpu_bgv_encoder_destroy": [vp],
+            "lgpu_bgv_encode": [vp, vp, i, i, u64, i, vp, i, vp, i, z, z, z, vp],
+            "lgpu_bgv_decode": [vp, vp, i, i, u64, vp, i, z, z, vp],
             "lgpu_poly_load": [vp, vp, z, vp, i, vp, vp, vp],
             "lgpu_poly_store": [vp, vp, i, vp, z, vp, vp],
             "lgpu_gadget_ct_load": [vp, vp, z, vp, z, vp, vp],
@@ -114,10 +118,11 @@ def lib():
         for name, args in sig.items():
             f = getattr(L, name)
             f.argtypes = args
-            if name not in ("lgpu_destroy", "lgpu_bgv_destroy"):
+            if name not in ("lgpu_destroy", "lgpu_bgv_destroy", "lgpu_bgv_encoder_destroy"):
                 f.restype = i
         L.lgpu_destroy.restype = None
         L.lgpu_bgv_destroy.restype = None
+        L.lgpu_bgv_encoder_destroy.restype = None
         L.lgpu_galois_element.restype = c.c_uint64
         L.lgpu_galois_element.argtypes = [vp, c.c_longlong]
         L.lgpu_launch_count.restype = c.c_ulonglong

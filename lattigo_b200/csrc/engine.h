@@ -143,6 +143,8 @@ int ensure_scratch(Ctx* c, size_t words);
 int upload_limb_tables(Ctx* c, int g);
 // half modulus of the product of `mods[0..n)` reduced mod m: floor(prod/2) mod m
 u64 h_half_prod_mod(const u64* mods, int n, u64 m);
+// GenModUpConstants(S[0..nS), T[0..nT)) appended to `blob`; the returned offsets index it (layout in ModUpSet)
+ModUpSet gen_modup(std::vector<u64>& blob, const u64* S, int nS, const u64* T, int nT);
 
 // ---- launchers (ntt.cu / vecops.cu / basisext.cu / keyswitch.cu) ---------------------------------------
 // All launchers are asynchronous on `st`. rows: RowMap; data: base pointer, row stride, batch count/stride.

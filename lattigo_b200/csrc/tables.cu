@@ -148,7 +148,7 @@ u64 h_half_prod_mod(const u64* mods, int n, u64 m) {
 }
 
 // GenModUpConstants (ring/basis_extension.go:101-172) appended to the blob.
-static ModUpSet gen_modup(std::vector<u64>& blob, const u64* S, int nS, const u64* T, int nT) {
+ModUpSet gen_modup(std::vector<u64>& blob, const u64* S, int nS, const u64* T, int nT) {
     ModUpSet m;
     m.nS = nS; m.nT = nT;
     m.off_qoverqiinvqi = blob.size();
