@@ -579,6 +579,23 @@ void lgpu_bgv_destroy(lgpu_bgv* ev);
  * each Rescale, and to MulScaleInvariant(s_a, s_b, level) = s_a * s_b / (-Q_level mod t) for BFV (:983-989). */
 int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const uint64_t* ct_b, const lgpu_gadget_ct* rlk,
                             int scale_invariant, int nb_rescales, uint64_t* ct_out, int batch, void* stream);
+/* bgv polynomial.Evaluator.Evaluate (circuits/bgv/polynomial/polynomial_evaluator.go:38-51) of one polynomial on a batch: the program
+ * format of lgpu_ckks_polynomial_evaluate, planned by lattigo_b200/bgv_polyeval.py (power basis, Paterson-Stockmeyer split, the BGV
+ * simEvaluator, and the schemes/bgv Add / MulThenAdd / Mul scale rules mod t folded into the weights). The ops, for the BGV evaluator
+ * (scale_invariant = 0, tensorStandard) or the BFV one (scale_invariant = 1, tensorScaleInvariant: the evaluator's ScaleInvariant):
+ *   MULRELIN dst = MulRelinNew(src0, src1)                 tensorStandard or tensorScaleInvariant, then relinearization
+ *   TENSOR   dst = r_b Mul(src0, src1) + r_a addend        Mul without relinearization (same tensor), then Add: r_b = r_a = 1, or
+ *                                                           matchScalesBinary's (r0, r1) when the scales differ
+ *   RELIN    dst = Relinearize(src0)
+ *   RESCALE  dst = Rescale(src0)                            DivRoundByLastModulusNTT; levels_per_rescale must be 1
+ *   LINCOMB  as for CKKS; the planner gives both NTT halves the same weights
+ * ct_in [batch][2][level+1][N] (NTT domain) -> ct_out [batch][2][level_out+1][N]. Checked before any launch, also on a host-only
+ * handle: everything lgpu_ckks_polynomial_evaluate checks, a non-null ev, scale_invariant 0 or 1, levels_per_rescale == 1, no RESCALE
+ * when scale_invariant, scale-invariant MULRELIN / TENSOR operands at the op's level, and rlk at every MULRELIN / RELIN level. The
+ * output scale and level are the planner's. Scratch as lgpu_ckks_polynomial_evaluate, plus the QMul buffers of one
+ * tensorScaleInvariant for BFV. */
+int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                 const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out, void* stream);
 
 
 /* ---- BGV / BFV encoder (schemes/bgv/encoder.go; BFV uses the same bgv.Encoder) ---------------------------------------

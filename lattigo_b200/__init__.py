@@ -17,3 +17,4 @@ from . import encryptor  # noqa: F401,E402
 from . import ckks_fft  # noqa: F401,E402
 from .encoder import Encoder  # noqa: F401,E402
 from .bgv_encoder import BGVEncoder  # noqa: F401,E402
+from .bgv_polyeval import BGVPolynomialEvaluator  # noqa: F401,E402

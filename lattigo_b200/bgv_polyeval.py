@@ -1,0 +1,208 @@
+"""bgv polynomial.Evaluator.Evaluate (circuits/bgv/polynomial/polynomial_evaluator.go:38-51) on the device: one bignum.Polynomial in the
+monomial basis with uint64 coefficients (Lead = true, Lazy = false), a batch of degree-1 NTT-domain ciphertexts sharing one level and
+scale, for the BGV evaluator (InvariantTensoring = false) or the BFV one (InvariantTensoring = true, the evaluator's ScaleInvariant).
+
+The scheme-independent planning (power basis, SplitDegree, OptimalSplit, Factorize, the Paterson-Stockmeyer recursion, the giant-step
+loop, the program format) is lattigo_b200/polyeval.py's; this module adds the BGV parts:
+  - the BGV simEvaluator (polynomial_evaluator_sim.go): PolynomialDepth, Rescale, MulNew and the baby / giant step updates in both
+    tensoring modes, including -Q_level mod t for BFV;
+  - rlwe.Scale with Mod = t (core/rlwe/scale.go:77-119): Mul and Div are exact mod t, Cmp compares the values; here Python ints;
+  - the schemes/bgv rules folded into the LINCOMB weights: Add(res, c0) as c0 scale mod t, centred, times tInvModQ[level]
+    (evaluator.go:142-172), and MulThenAdd(X^k, c, res) with the op0.Scale / opOut.Scale ratio mod t, centred (:1088-1141);
+  - Mul / MulRelin dispatching on ScaleInvariant (:391-396, :529-532, MulScaleInvariant :983-989) and Rescale, a no-op for BFV
+    (:1363-1393).
+EvaluateMonomial checks a.Scale.InDelta(b.Scale, ScalePrecision - 12) before its Add. Scales mod t are integers below 2^64, so that
+check passes only when they are equal, and the Add never reaches matchScalesBinary: every TENSOR has r_b = r_a = 1."""
+from __future__ import annotations
+
+import ctypes
+from typing import Sequence
+
+from . import _lib
+from .polyeval import CHEBYSHEV, MONOMIAL, MULRELIN, RESCALE, TENSOR, Program, _Lin, _Planner, _Poly, _Sim, _Sym
+from .ring import _dptr, _stream
+
+U64_MAX = (1 << 64) - 1
+
+
+class ScaleModT:
+    """rlwe.Scale with Mod = t on integer values (core/rlwe/scale.go:77-119)."""
+
+    def __init__(self, t: int):
+        self.t = t
+
+    def mul(self, a: int, b: int) -> int:
+        return a * b % self.t
+
+    def div(self, a: int, b: int) -> int:
+        try:
+            inv = pow(b, -1, self.t)
+        except ValueError:                       # big.Int.ModInverse leaves its receiver unchanged when there is no inverse
+            inv = b
+        return a * inv % self.t
+
+
+def q_mod_t_neg(Q: Sequence[int], level: int, t: int) -> int:
+    """T - (ModulusAtLevel[level] mod T), the factor of MulScaleInvariant and of the BFV giant step."""
+    prod = 1
+    for q in Q[: level + 1]:
+        prod *= q
+    return t - prod % t
+
+
+def centred(c: int, t: int) -> int:
+    """c mod T (Euclidean), minus T above T/2 (the scalar cases of Add / Mul / MulThenAdd)."""
+    c %= t
+    return c - t if c > t >> 1 else c
+
+
+class _BGVSim(_Sim):                              # circuits/bgv/polynomial/polynomial_evaluator_sim.go
+    def __init__(self, Q, t, si):
+        super().__init__(Q, 1)
+        self.t, self.si, self.S = t, si, ScaleModT(t)
+
+    def depth(self, degree):
+        if self.si:
+            return 0
+        if degree <= 0:
+            raise ValueError("invalid degree: degree=%d should be greater than zero" % degree)
+        return degree.bit_length() - 1
+
+    def rescale(self, lv, s):
+        if self.si:
+            return lv, s
+        return lv - 1, self.S.div(s, self.Q[lv])
+
+    def mul(self, a, b):
+        lv = min(a[0], b[0])
+        s = self.S.mul(a[1], b[1])
+        return lv, self.S.div(s, q_mod_t_neg(self.Q, lv, self.t)) if self.si else s
+
+    def same_scale(self, a, b):                  # InDelta(.., 116) on integers below 2^64 is equality
+        return a == b
+
+    def baby(self, lead, lv, s):
+        if not self.si and lead:
+            s = self.S.mul(s, self.Q[lv])
+        return lv, s
+
+    def giant(self, lead, lv, s, xs):
+        s = self.S.div(s, xs)
+        if self.si:
+            return lv, self.S.mul(s, q_mod_t_neg(self.Q, lv, self.t))
+        return lv + 1, self.S.mul(s, self.Q[lv] if lead else self.Q[lv + 1])
+
+
+class _BGVPlanner(_Planner):
+    def __init__(self, Q, t, si):
+        super().__init__(Q, 1, 64, None)
+        self.t, self.si = t, si
+        self.sim = _BGVSim(self.Q, t, si)
+
+    def _sim(self):
+        return self.sim
+
+    # ---- rounding ops --------------------------------------------------------------------------------------------
+    def rescale(self, x: _Sym) -> _Sym:          # Rescale (:1363-1393): DivRoundByLastModulusNTT, or nothing for BFV
+        if self.si:
+            return x
+        if x.level == 0:
+            raise ValueError("cannot rescale: op0 already at level 0")
+        y = _Sym(self._slot(), x.level - 1, self.sim.S.div(x.scale, self.Q[x.level]), x.deg)
+        self.prog.ops.append(dict(kind=RESCALE, dst=y.slot, src0=x.slot, level=y.level))
+        return y
+
+    def mul_relin(self, a: _Sym, b: _Sym) -> _Sym:
+        lv, s = self.sim.mul((a.level, a.scale), (b.level, b.scale))
+        y = _Sym(self._slot(), lv, s, 1)
+        self.prog.ops.append(dict(kind=MULRELIN, dst=y.slot, src0=a.slot, src1=b.slot, level=lv))
+        return y
+
+    def baby_step(self, pol, pb, level, scale) -> _Lin:
+        if pol.IsEven and not pol.IsOdd and pol.Degree() == 0:
+            # NewCiphertext(params, 0, level): Mul(b, X^k) then takes the plaintext branch of tensorStandard, which reads X^k's first
+            # component only (BGV), and tensorScaleInvariant indexes a second component that is not there (BFV)
+            raise ValueError("an even-only polynomial whose giant-step quotient is a constant gives a degree-0 baby step, which the "
+                             "reference's Mul does not multiply as a ciphertext; not supported")
+        return super().baby_step(pol, pb, level, scale)
+
+    def monomial(self, a: _Sym, b: _Sym, x: _Sym) -> _Sym:      # EvaluateMonomial: Mul(b, X^k) + Add(.., a) as one TENSOR
+        if b.deg == 2:
+            b = self.relin(b)
+        b = self.rescale(b)
+        lv, bs = self.sim.mul((b.level, b.scale), (x.level, x.scale))
+        if not self.sim.same_scale(a.scale, bs):
+            raise ValueError("evalMonomial: scale discrepency: (rescale(b) * X^{n}).Scale = %d != a.Scale = %d" % (bs, a.scale))
+        lv = min(lv, a.level)
+        y = _Sym(self._slot(), lv, bs, 2)
+        self.prog.ops.append(dict(kind=TENSOR, dst=y.slot, src0=b.slot, src1=x.slot, addend=a.slot, level=lv, weights=[1] * (2 * (lv + 1))))
+        return y
+
+    # ---- schemes/bgv linear ops, folded ----------------------------------------------------------------------
+    def add_const(self, f: _Lin, c: int):        # Add(ct, uint64): AddScalarBigint of c scale T^-1 on component 0
+        Ql = 1
+        for q in self.Q[: f.level + 1]:
+            Ql *= q
+        v = centred(c * f.scale, self.t) * pow(self.t, -1, Ql)
+        for i, q in enumerate(self.Q[: f.level + 1]):
+            f.const[i] = [(f.const[i][h] + v) % q for h in range(2)]
+
+    def mul_then_add(self, x: _Sym, c: int, f: _Lin):         # MulThenAdd(X^k, uint64, res): MulScalarBigintThenAdd
+        if x.scale != f.scale:
+            ratio = pow(x.scale, self.t - 2, self.t) * f.scale % self.t
+            c = c * ratio
+        v = centred(c, self.t)
+        cur = f.w.get(x.slot) or [[0, 0] for _ in range(f.level + 1)]
+        # rows above X^k's level are not written (the ring runs at min(op0.Level(), opOut.Level()))
+        f.w[x.slot] = [[(cur[i][h] + (v if i <= x.level else 0)) % q for h in range(2)] for i, q in enumerate(self.Q[: f.level + 1])]
+
+
+def plan(Q: Sequence[int], t: int, level: int, scale: int, coeffs: Sequence[int], target_scale: int, scale_invariant: bool = False,
+         odd: bool = True, even: bool = True, basis: int = MONOMIAL) -> Program:
+    """The device program of Evaluate(ct, bignum.NewPolynomial(Monomial, coeffs, nil) with IsOdd = odd, IsEven = even, targetScale) for a
+    ciphertext at `level` with rlwe.Scale `scale` (Mod = t); scale_invariant is the evaluator's ScaleInvariant (InvariantTensoring)."""
+    if basis == CHEBYSHEV:
+        raise ValueError("the Chebyshev basis is not supported for BGV polynomial evaluation (uint64 coefficients); use the monomial basis")
+    if basis != MONOMIAL:
+        raise ValueError("basis must be MONOMIAL")
+    coeffs = [int(c) for c in coeffs]
+    if any(c < 0 or c > U64_MAX for c in coeffs):
+        raise ValueError("coefficients must be uint64")
+    t = int(t)
+    for name, s in (("scale", scale), ("target_scale", target_scale)):
+        if not 1 <= int(s) < t:
+            raise ValueError("%s must be an integer in [1, t)" % name)
+    p = _Poly(list(coeffs), MONOMIAL, odd, even)
+    if p.Degree() > 255:
+        raise ValueError("degree %d > 255 is not supported" % p.Degree())
+    return _BGVPlanner(Q, t, bool(scale_invariant)).evaluate(level, int(scale), p, int(target_scale))
+
+
+class BGVPolynomialEvaluator:
+    """polynomial.Evaluator (circuits/bgv/polynomial) over a BGVEvaluator: InvariantTensoring = bgv_evaluator.ScaleInvariant."""
+
+    def __init__(self, bgv_evaluator):
+        self.ev = bgv_evaluator
+        self.ctx = bgv_evaluator.ctx
+        self.InvariantTensoring = bgv_evaluator.ScaleInvariant
+
+    def plan(self, level, scale, coeffs, target_scale, odd=True, even=True, basis=MONOMIAL) -> Program:
+        return plan(self.ctx.Q, self.ev.t, level, scale, coeffs, target_scale, self.InvariantTensoring, odd, even, basis)
+
+    def Evaluate(self, ct, scale, coeffs, target_scale, odd=True, even=True, basis=MONOMIAL):
+        """ct: (batch, 2, level+1, N) or (2, level+1, N) int64 CUDA tensor, NTT domain. Returns (ct_out, level, scale)."""
+        import torch
+        level = ct.shape[-2] - 1
+        prog = self.plan(level, scale, coeffs, target_scale, odd, even, basis)
+        b = ct.shape[0] if ct.dim() == 4 else 1
+        shape = (b, 2, prog.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prog.out_level + 1, self.ctx.N)
+        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
+        self.run(prog, ct, out, b)
+        return out, prog.out_level, prog.out_scale
+
+    def run(self, prog: Program, ct, out, batch: int):
+        cp = prog.to_c(1)
+        rlk = self.ev.rlk
+        _lib.check(_lib.lib().lgpu_bgv_polynomial_evaluate(self.ev.h, ct.shape[-2] - 1, _dptr(ct), batch, ctypes.byref(cp),
+                                                           rlk.ref() if rlk is not None else None, 1 if self.InvariantTensoring else 0,
+                                                           _dptr(out), _stream()))

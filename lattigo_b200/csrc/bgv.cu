@@ -15,23 +15,11 @@
 #include <algorithm>
 #include <cstring>
 #include <vector>
-#include "capi_common.h"
+#include "bgv.h"
 #include "composite.h"
 #include "modarith.cuh"
 
 namespace lgpu {
-
-struct BgvState {
-    Ctx qm;                          // (Q, QMul): Q limbs 0..nQ-1, QMul limbs nQ..nQ+nQMul-1
-    u64 t = 0;
-    std::vector<int> levelQMul;      // [level of Q]
-    std::vector<size_t> lvl_off;     // [level of Q]: offset (words) of that level's quantize block in d_const
-    // d_const: tmul[nQ] = MForm(t mod q_i) | tmont[nQ] = MForm(t 2^64 mod q_i) (tMontgomery) | per-level blocks:
-    //   half1_s[nq]: floor(Q_l/2) mod q_i   half2_t[nq]: floor(QMul_lm/2) mod q_i   half1_t[nm]: floor(Q_l/2) mod p_j
-    //   mdcs[nm]: p_j - modDownConstantsQtoP[l][j]   half2_s[nm]: floor(QMul_lm/2) mod p_j          (nm = levelQMul[l] + 1)
-    std::vector<u64> h_const;
-    u64* d_const = nullptr;
-};
 
 // ---------------------------------------------------------------------------------------------------------
 // Tensor
@@ -257,23 +245,20 @@ static int bgv_chunk(const Ctx* c, const BgvState& s, int level, const u64* A, c
     RnsTensorParams p = tensor_params(c->d_limbs, c->N);
     p.rm = rows_range(0, 0, (int)nq); p.nq = (int)nq;
     p.seg[0] = TensorSeg{A, B, nq * N, 2 * nq * N, buf.p, (size_t)batch * nq * N, nq * N};
-    p.pre = s.d_const + c->nQ;   // tmont
+    p.pre = s.tmont();
     if (launch_rns_tensor(p, true, A == B, batch, st)) return -1;
     return mulrelin_tail(c, level, buf.p, rlk, nb_rescales, out, batch, st);
 }
 
-// tensorScaleInvariant with relinearization
-static int bfv_chunk(const Ctx* c, const BgvState& s, int level, const u64* A, const u64* B, const GadgetCt& rlk, u64* out, int batch,
-                     cudaStream_t st) {
+// tensorScaleInvariant up to the degree-2 product (bgv.h)
+int bfv_tensor(const Ctx* c, const BgvState& s, int level, const u64* A, const u64* B, u64* d, int batch, cudaStream_t st) {
     const Ctx* m = &s.qm;
     const int lm = s.levelQMul[level];
     const size_t N = c->N, nq = level + 1, nm = lm + 1;
     const bool square = A == B;
-    Scratch buf, mbuf;
-    if (buf.alloc((size_t)batch * 5 * nq * N, st)) return -1;             // d0, d1, d2, t0, t1 (t0|t1: INTT of one operand)
+    Scratch mbuf;
     if (mbuf.alloc((size_t)batch * 7 * nm * N, st)) return -1;            // QMul: extA [2], extB [2], products [3]
-    u64* d = buf.p;
-    u64* tmp = d + (size_t)3 * batch * nq * N;
+    u64* tmp = d + (size_t)3 * batch * nq * N;                             // INTT of one operand
     u64* ext[2] = {mbuf.p, mbuf.p + (size_t)2 * batch * nm * N};
     u64* dm = mbuf.p + (size_t)4 * batch * nm * N;
     const RowMap rq = rows_range(0, 0, (int)nq), rmul = rows_range(m->nQ, 0, (int)nm);
@@ -305,8 +290,16 @@ static int bfv_chunk(const Ctx* c, const BgvState& s, int level, const u64* A, c
     q.c1_cinv = u1.off_qoverqiinvqi; q.c1_c = u1.off_qoverqimodp; q.c1_v = u1.off_vtimesqmodp;
     q.c2_cinv = u2.off_qoverqiinvqi; q.c2_c = u2.off_qoverqimodp; q.c2_v = u2.off_vtimesqmodp;
     if (launch_quantize(q, 3 * batch, st)) return -1;
-    if (launch_ntt(c, rq, CSpan{d, N, nq * N}, Span{d, N, nq * N}, 3 * batch, NTT_CANONICAL, st)) return -1;
-    return mulrelin_tail(c, level, d, rlk, 0, out, batch, st);
+    return launch_ntt(c, rq, CSpan{d, N, nq * N}, Span{d, N, nq * N}, 3 * batch, NTT_CANONICAL, st);
+}
+
+// tensorScaleInvariant with relinearization
+static int bfv_chunk(const Ctx* c, const BgvState& s, int level, const u64* A, const u64* B, const GadgetCt& rlk, u64* out, int batch,
+                     cudaStream_t st) {
+    Scratch buf;
+    if (buf.alloc((size_t)batch * 5 * (level + 1) * c->N, st)) return -1;   // d0, d1, d2, t0, t1
+    if (bfv_tensor(c, s, level, A, B, buf.p, batch, st)) return -1;
+    return mulrelin_tail(c, level, buf.p, rlk, 0, out, batch, st);
 }
 
 // number of bits of prod(mods[0..n)), as big.Int.BitLen
@@ -325,11 +318,6 @@ static int prod_bitlen(const u64* mods, int n) {
 }
 
 }  // namespace lgpu
-
-struct lgpu_bgv {
-    lgpu_ctx* ctx = nullptr;
-    lgpu::BgvState s;
-};
 
 using namespace lgpu;
 

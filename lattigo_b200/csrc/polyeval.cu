@@ -1,14 +1,19 @@
-// polyeval.cu -- ckks polynomial.Evaluator.Evaluate (circuits/ckks/polynomial/polynomial_evaluator.go:42-57) for a BATCH of ciphertexts,
-// running a program planned on the host (lattigo_b200/polyeval.py): MULRELIN / TENSOR / RELIN / RESCALE / LINCOMB ops over
-// single-assignment slots (include/lattigo_b200.h). Two kernels are new:
-//   poly_lincomb_kernel  every baby step of a call (or one Chebyshev power combine) in one pass that reads each power once;
-//   poly_tensor_kernel   EvaluateMonomial's Mul(b, X^k) + Add(.., a) with the scale ratios, in one pass (also the tensor of MULRELIN).
-// Relinearization, the key switch of MulRelinNew and Rescale use the existing launchers. Every op's output is the canonical residue of a
-// linear combination of canonical inputs, so the results equal the reference's op-by-op sequence bit for bit (DESIGN 3.4;
-// tests/test_gpu_polyeval.py vs oracle/polyeval.py).
+// polyeval.cu -- ckks and bgv polynomial.Evaluator.Evaluate (circuits/ckks/polynomial/polynomial_evaluator.go:42-57,
+// circuits/bgv/polynomial/polynomial_evaluator.go:38-51) for a BATCH of ciphertexts, running a program planned on the host
+// (lattigo_b200/polyeval.py, lattigo_b200/bgv_polyeval.py): MULRELIN / TENSOR / RELIN / RESCALE / LINCOMB ops over
+// single-assignment slots (include/lattigo_b200.h). The kernels:
+//   poly_lincomb_kernel     every baby step of a call (or one Chebyshev power combine) in one pass that reads each power once;
+//   poly_tensor_kernel      EvaluateMonomial's Mul(b, X^k) + Add(.., a) with the scale ratios, in one pass (also the tensor of
+//                           MULRELIN); TMUL pre-multiplies b by tMontgomery (BGV tensorStandard) instead of MForm (CKKS);
+//   poly_tensor_add_kernel  the same Add on a product that is already in memory (BFV: the scale-invariant tensor of bgv.cu).
+// Only MULRELIN and TENSOR depend on the scheme (Runner::mulrelin / Runner::tensor_op). Relinearization, the key switch of
+// MulRelinNew and Rescale use the existing launchers. Every op's output is the canonical residue of a linear combination of canonical
+// inputs, so the results equal the reference's op-by-op sequence bit for bit (DESIGN 3.4; tests/test_gpu_polyeval.py vs
+// oracle/polyeval.py, tests/test_gpu_bgv_polyeval.py vs tests/bgv_polyeval_oracle.py).
 #include <algorithm>
+#include <cstring>
 #include <vector>
-#include "capi_common.h"
+#include "bgv.h"
 #include "composite.h"
 #include "modarith.cuh"
 
@@ -85,11 +90,27 @@ struct PolyTensorParams {
     const u64* wb; const u64* wa;        // MForm(r_b), MForm(r_a) per limb (ADD only)
     u64* d; size_t d_cs, d_bs;           // degree 2
     int n;
+    const u64* tmont;                    // TMUL: tMontgomery per limb
 };
+
+// d_c = MRed(x_c, MForm(r_b)) (+) MRed(a_c, MForm(r_a)) for c = 0..2, the addend's components up to a_deg
+__device__ __forceinline__ void poly_add_epilogue(const PolyTensorParams& p, const u64 (&x)[3], int r, size_t b, size_t ro, u64 q, u64 qinv) {
+    const u64 wb = p.wb[r], wa = p.wa[r];
+    const u64* A = p.a + b * p.a_bs + ro;
+    u64* D = p.d + b * p.d_bs + ro;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        u64 v = mred(x[c], wb, q, qinv);
+        if (c <= p.a_deg) v = cred(v + mred(A[c * p.a_cs], wa, q, qinv), q);
+        D[c * p.d_cs] = v;
+    }
+}
 // schemes/ckks/evaluator.go:807-820 (c00 = MForm(b0), c01 = MForm(b1); d0 = MRed(c00, x0), d2 = MRed(c01, x1),
 // d1 = MRed(c00, x1) (+) MRed(c01, x0)), then, with ADD, d_c = MRed(d_c, MForm(r_b)) (+) MRed(a_c, MForm(r_a)) (the Mul by the
 // truncated scale ratio and the Add of EvaluateMonomial, :238-246 and evaluateInPlace :221-408). All canonical.
-template <bool ADD>
+// TMUL: c00 = MRed(b0, tMontgomery), c01 = MRed(b1, tMontgomery) (schemes/bgv/evaluator.go:634-635), then the same products and Add
+// (r_b, r_a: 1 or matchScalesBinary's r0, r1, :210-227).
+template <bool ADD, bool TMUL>
 __global__ void __launch_bounds__(256) poly_tensor_kernel(PolyTensorParams p) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= p.n) return;
@@ -99,26 +120,38 @@ __global__ void __launch_bounds__(256) poly_tensor_kernel(PolyTensorParams p) {
     const size_t b = blockIdx.z, ro = (size_t)r * p.n + j;
     const u64* B = p.b + b * p.b_bs + ro;
     const u64* X = p.x + b * p.x_bs + ro;
-    const u64 m0 = mform(B[0], q, L.bred_hi, L.bred_lo), m1 = mform(B[p.b_cs], q, L.bred_hi, L.bred_lo);
+    u64 m0, m1;
+    if (TMUL) {
+        const u64 tm = p.tmont[r];
+        m0 = mred(B[0], tm, q, qinv); m1 = mred(B[p.b_cs], tm, q, qinv);
+    } else {
+        m0 = mform(B[0], q, L.bred_hi, L.bred_lo); m1 = mform(B[p.b_cs], q, L.bred_hi, L.bred_lo);
+    }
     const u64 x0 = X[0], x1 = X[p.x_cs];
     u64 d[3];
     d[0] = mred(m0, x0, q, qinv);
     d[2] = mred(m1, x1, q, qinv);
     d[1] = cred(mred(m0, x1, q, qinv) + mred(m1, x0, q, qinv), q);
-    u64* D = p.d + b * p.d_bs + ro;
     if (ADD) {
-        const u64 wb = p.wb[r], wa = p.wa[r];
-        const u64* A = p.a + b * p.a_bs + ro;
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            u64 v = mred(d[c], wb, q, qinv);
-            if (c <= p.a_deg) v = cred(v + mred(A[c * p.a_cs], wa, q, qinv), q);
-            D[c * p.d_cs] = v;
-        }
+        poly_add_epilogue(p, d, r, b, ro, q, qinv);
     } else {
+        u64* D = p.d + b * p.d_bs + ro;
 #pragma unroll
         for (int c = 0; c < 3; c++) D[c * p.d_cs] = d[c];
     }
+}
+
+// The Add of EvaluateMonomial on a degree-2 product x already in memory (p.b, components b_cs apart): BFV, whose scale-invariant
+// tensor (bfv_tensor) ends with an NTT pass and so cannot carry the epilogue.
+__global__ void __launch_bounds__(256) poly_tensor_add_kernel(PolyTensorParams p) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= p.n) return;
+    const int r = blockIdx.y;
+    const LimbConst L = p.limbs[r];
+    const size_t b = blockIdx.z, ro = (size_t)r * p.n + j;
+    const u64* X = p.b + b * p.b_bs + ro;
+    const u64 x[3] = {X[0], X[p.b_cs], X[2 * p.b_cs]};
+    poly_add_epilogue(p, x, r, b, ro, L.q, L.qinv);
 }
 
 namespace {
@@ -251,6 +284,8 @@ struct Runner {
     std::vector<Slot> s;
     const u64* d_w;                       // all op weights, uploaded once
     std::vector<size_t> w_off;
+    const BgvState* bgv = nullptr;        // BGV / BFV: the evaluator state; null for CKKS
+    bool si = false;                      // BFV: scale-invariant tensoring
 
     size_t cs(int i) const { return (size_t)(s[i].level + 1) * c->N; }
     size_t bs(int i) const { return (size_t)(s[i].deg + 1) * cs(i); }
@@ -276,10 +311,52 @@ struct Runner {
         p.a = asl >= 0 ? s[asl].p : nullptr; p.a_cs = asl >= 0 ? cs(asl) : 0; p.a_bs = asl >= 0 ? bs(asl) : 0; p.a_deg = asl >= 0 ? s[asl].deg : -1;
         p.wb = w; p.wa = w ? w + (level + 1) : nullptr;
         p.d = d; p.d_cs = d_cs; p.d_bs = d_bs; p.n = c->N;
+        p.tmont = bgv ? bgv->tmont() : nullptr;
         ProfScope ps(LGPU_KCLASS_TENSOR, st, 8.0 * c->N * (level + 1) * nb * (w ? 7 + (p.a_deg + 1) : 7), 1);
         const dim3 grid((c->N + 255) / 256, (unsigned)(level + 1), (unsigned)nb);
-        if (w) poly_tensor_kernel<true><<<grid, 256, 0, st>>>(p);
-        else poly_tensor_kernel<false><<<grid, 256, 0, st>>>(p);
+        if (bgv) {
+            if (w) poly_tensor_kernel<true, true><<<grid, 256, 0, st>>>(p);
+            else poly_tensor_kernel<false, true><<<grid, 256, 0, st>>>(p);
+        } else {
+            if (w) poly_tensor_kernel<true, false><<<grid, 256, 0, st>>>(p);
+            else poly_tensor_kernel<false, false><<<grid, 256, 0, st>>>(p);
+        }
+        LGPU_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+
+    // MulRelinNew of two degree-1 slots into the degree-1 slot dst (made by the caller): the scheme's tensor, then mulrelin_tail
+    int mulrelin(const lgpu_poly_op& o) {
+        const size_t N = c->N, nq = o.level + 1;
+        Scratch buf;                                   // d0, d1, d2, t0, t1: [5][nb][nq][N] (mulrelin_tail's layout)
+        if (buf.alloc((size_t)nb * 5 * nq * N, st)) return -1;
+        if (si) {
+            if (bfv_tensor(c, *bgv, o.level, s[o.src0].p, s[o.src1].p, buf.p, nb, st)) return -1;
+        } else if (tensor(o.src0, o.src1, -1, nullptr, o.level, buf.p, (size_t)nb * nq * N, nq * N)) {
+            return -1;
+        }
+        return mulrelin_tail(c, o.level, buf.p, rlk, 0, s[o.dst].p, nb, st);
+    }
+
+    // TENSOR of op i into its degree-2 slot dst (made by the caller)
+    int tensor_op(int i) {
+        const lgpu_poly_op& o = pg->ops[i];
+        const u64* w = d_w + w_off[i];
+        if (!si) return tensor(o.src0, o.src1, o.addend, w, o.level, s[o.dst].p, cs(o.dst), bs(o.dst));
+        const size_t N = c->N, nq = o.level + 1;
+        Scratch buf;                                   // the product [3][nb][nq][N] and bfv_tensor's scratch
+        if (buf.alloc((size_t)nb * 5 * nq * N, st)) return -1;
+        if (bfv_tensor(c, *bgv, o.level, s[o.src0].p, s[o.src1].p, buf.p, nb, st)) return -1;
+        const int a = o.addend;
+        PolyTensorParams p;
+        memset(&p, 0, sizeof(p));
+        p.limbs = c->d_limbs;
+        p.b = buf.p; p.b_cs = (size_t)nb * nq * N; p.b_bs = nq * N;
+        p.a = a >= 0 ? s[a].p : nullptr; p.a_cs = a >= 0 ? cs(a) : 0; p.a_bs = a >= 0 ? bs(a) : 0; p.a_deg = a >= 0 ? s[a].deg : -1;
+        p.wb = w; p.wa = w + nq;
+        p.d = s[o.dst].p; p.d_cs = cs(o.dst); p.d_bs = bs(o.dst); p.n = c->N;
+        ProfScope ps(LGPU_KCLASS_VECOP, st, 8.0 * N * nq * nb * (6 + (p.a_deg + 1)), 1);
+        poly_tensor_add_kernel<<<dim3((c->N + 255) / 256, (unsigned)nq, (unsigned)nb), 256, 0, st>>>(p);
         LGPU_CUDA_OK(cudaGetLastError());
         return 0;
     }
@@ -288,17 +365,12 @@ struct Runner {
         const lgpu_poly_op& o = pg->ops[i];
         const size_t N = c->N;
         switch (o.kind) {
-        case LGPU_POLY_MULRELIN: {
+        case LGPU_POLY_MULRELIN:
             if (make(o.dst, o.dst == pg->out_slot ? out_chunk : nullptr)) return -1;
-            const size_t nq = o.level + 1;
-            Scratch buf;                                   // d0, d1, d2, t0, t1: [5][nb][nq][N] (mulrelin_tail's layout)
-            if (buf.alloc((size_t)nb * 5 * nq * N, st)) return -1;
-            if (tensor(o.src0, o.src1, -1, nullptr, o.level, buf.p, (size_t)nb * nq * N, nq * N)) return -1;
-            return mulrelin_tail(c, o.level, buf.p, rlk, 0, s[o.dst].p, nb, st);
-        }
+            return mulrelin(o);
         case LGPU_POLY_TENSOR:
             if (make(o.dst, nullptr)) return -1;
-            return tensor(o.src0, o.src1, o.addend, d_w + w_off[i], o.level, s[o.dst].p, cs(o.dst), bs(o.dst));
+            return tensor_op(i);
         case LGPU_POLY_RELIN: {
             if (make(o.dst, o.dst == pg->out_slot ? out_chunk : nullptr)) return -1;
             const int a = o.src0, d = o.dst;
@@ -335,6 +407,46 @@ struct Runner {
     }
 };
 
+
+// the relinearization key, checked at every level a MULRELIN / RELIN uses it
+int program_rlk(const Ctx& c, const lgpu_poly_program* prog, const lgpu_gadget_ct* rlk, GadgetCt& g) {
+    bool needs_rlk = false;
+    for (int i = 0; i < prog->n_ops; i++) needs_rlk |= prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN;
+    if (!needs_rlk) return 0;
+    if (to_gadget_ct(rlk, g, "null relinearization key")) return -1;
+    for (int i = 0; i < prog->n_ops; i++)
+        if ((prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN) && check_evk(&c, prog->ops[i].level, g)) return -1;
+    return 0;
+}
+
+// runs a validated program over the batch, one batch_chunk() sub-batch at a time
+int run_program(const Ctx& c, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog, const Plan& pl, const GadgetCt& g,
+                const BgvState* bgv, bool si, uint64_t* ct_out, cudaStream_t st) {
+    std::vector<u64> hw;
+    std::vector<size_t> off(prog->n_ops, 0);
+    for (int i = 0; i < prog->n_ops; i++) { off[i] = hw.size(); hw.insert(hw.end(), pl.w[i].begin(), pl.w[i].end()); }
+    Scratch dw;
+    if (!hw.empty()) {
+        if (dw.alloc(hw.size(), st)) return -1;
+        // pageable source: the call returns once `hw` is staged, so it may die with this function
+        LGPU_CUDA_OK(cudaMemcpyAsync(dw.p, hw.data(), hw.size() * 8, cudaMemcpyHostToDevice, st));
+    }
+    const size_t N = c.N, ci = (size_t)2 * (level + 1) * N, co = (size_t)2 * (pl.level[prog->out_slot] + 1) * N;
+    const int ch = batch_chunk();
+    for (int k = 0; k < batch; k += ch) {
+        const int nb = std::min(ch, batch - k);
+        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off, bgv, si};
+        R.s[0].p = (u64*)ct_in + (size_t)k * ci; R.s[0].deg = 1; R.s[0].level = level;
+        u64* out = (u64*)ct_out + (size_t)k * co;
+        for (int i = 0; i < prog->n_ops; i++) {
+            if (R.op(i, out)) return -1;
+            for (int sl = 1; sl < prog->n_slots; sl++)
+                if (pl.last_use[sl] == i && sl != prog->out_slot) R.release(sl);
+        }
+    }
+    return 0;
+}
+
 }  // namespace
 }  // namespace lgpu
 
@@ -352,36 +464,34 @@ extern "C" int lgpu_ckks_polynomial_evaluate(lgpu_ctx* ctx, int level, const uin
     Plan pl;
     if (validate(c, level, prog, pl)) return -1;
     GadgetCt g{};
-    bool needs_rlk = false;
-    for (int i = 0; i < prog->n_ops; i++) needs_rlk |= prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN;
-    if (needs_rlk) {
-        if (to_gadget_ct(rlk, g, "null relinearization key")) return -1;
-        for (int i = 0; i < prog->n_ops; i++)
-            if ((prog->ops[i].kind == LGPU_POLY_MULRELIN || prog->ops[i].kind == LGPU_POLY_RELIN) && check_evk(&c, prog->ops[i].level, g)) return -1;
-    }
+    if (program_rlk(c, prog, rlk, g)) return -1;
     REQUIRE_DEVICE(ctx);
-    const cudaStream_t st = (cudaStream_t)stream;
-    std::vector<u64> hw;
-    std::vector<size_t> off(prog->n_ops, 0);
-    for (int i = 0; i < prog->n_ops; i++) { off[i] = hw.size(); hw.insert(hw.end(), pl.w[i].begin(), pl.w[i].end()); }
-    Scratch dw;
-    if (!hw.empty()) {
-        if (dw.alloc(hw.size(), st)) return -1;
-        // pageable source: the call returns once `hw` is staged, so it may die with this function
-        LGPU_CUDA_OK(cudaMemcpyAsync(dw.p, hw.data(), hw.size() * 8, cudaMemcpyHostToDevice, st));
-    }
-    const size_t N = c.N, ci = (size_t)2 * (level + 1) * N, co = (size_t)2 * (pl.level[prog->out_slot] + 1) * N;
-    const int ch = batch_chunk();
-    for (int k = 0; k < batch; k += ch) {
-        const int nb = std::min(ch, batch - k);
-        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off};
-        R.s[0].p = (u64*)ct_in + (size_t)k * ci; R.s[0].deg = 1; R.s[0].level = level;
-        u64* out = (u64*)ct_out + (size_t)k * co;
+    return run_program(c, level, ct_in, batch, prog, pl, g, nullptr, false, ct_out, (cudaStream_t)stream);
+}
+
+extern "C" int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                            const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out, void* stream) {
+    REQUIRE(ev, "null BGV evaluator");
+    REQUIRE(scale_invariant == 0 || scale_invariant == 1, "scale_invariant must be 0 or 1");
+    const Ctx& c = ev->ctx->c;
+    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
+    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
+    REQUIRE(ct_in && ct_out, "null ciphertext");
+    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
+    Plan pl;
+    if (validate(c, level, prog, pl)) return -1;
+    REQUIRE(prog->levels_per_rescale == 1, "levels_per_rescale must be 1 for BGV / BFV (Rescale drops one modulus)");
+    if (scale_invariant) {
         for (int i = 0; i < prog->n_ops; i++) {
-            if (R.op(i, out)) return -1;
-            for (int sl = 1; sl < prog->n_slots; sl++)
-                if (pl.last_use[sl] == i && sl != prog->out_slot) R.release(sl);
+            const lgpu_poly_op& o = prog->ops[i];
+            REQUIRE(o.kind != LGPU_POLY_RESCALE, "the scale-invariant (BFV) evaluator does not rescale: RESCALE in a scale_invariant program");
+            // the scale-invariant tensor reads both operands as [batch][2][level+1][N]
+            REQUIRE(!(o.kind == LGPU_POLY_MULRELIN || o.kind == LGPU_POLY_TENSOR) || (pl.level[o.src0] == o.level && pl.level[o.src1] == o.level),
+                    "scale-invariant MULRELIN / TENSOR operands must be at the op's level");
         }
     }
-    return 0;
+    GadgetCt g{};
+    if (program_rlk(c, prog, rlk, g)) return -1;
+    REQUIRE_DEVICE(ev->ctx);
+    return run_program(c, level, ct_in, batch, prog, pl, g, &ev->s, scale_invariant == 1, ct_out, (cudaStream_t)stream);
 }

@@ -139,19 +139,31 @@ def _factorize(p: _Poly, n: int):                # bignum.Polynomial.Factorize +
 
 
 class _Sim:                                      # circuits/ckks/polynomial/polynomial_evaluator_sim.go
+    """The CKKS simEvaluator over (level, scale) pairs. gen_power and recurse are the scheme-independent SimPowerBasis.GenPower and
+    recursePS; a scheme's simEvaluator overrides depth, rescale, mul, baby, giant and same_scale."""
+
     def __init__(self, Q, lpr): self.Q, self.lpr = Q, lpr
+
+    def depth(self, degree):                     # PolynomialDepth
+        return self.lpr * (degree.bit_length() - 1)
 
     def rescale(self, lv, s):
         for _ in range(self.lpr):
             s = _sdiv(s, _snew(self.Q[lv])); lv -= 1
         return lv, s
 
+    def mul(self, a, b):                         # MulNew
+        return min(a[0], b[0]), _smul(a[1], b[1])
+
+    def same_scale(self, a, b):                  # Scale.InDelta(.., ScalePrecision - 12)
+        return _in_delta(a, b, SCALE_PREC - 12)
+
     def gen_power(self, pb, n):
         if n < 2:
             return
         a, b = split_degree(n)
         self.gen_power(pb, a); self.gen_power(pb, b)
-        pb[n] = self.rescale(min(pb[a][0], pb[b][0]), _smul(pb[a][1], pb[b][1]))
+        pb[n] = self.rescale(*self.mul(pb[a], pb[b]))
 
     def baby(self, lead, lv, s):
         if lead:
@@ -178,10 +190,9 @@ class _Sim:                                      # circuits/ckks/polynomial/poly
         cq, cr = _factorize(p, nextPower)
         tln, tsn = self.giant(p.Lead, tl, os_, xs)
         bq, res = self.recurse(logSplit, tln, cq, pb, tsn)
-        lv, s = self.rescale(*res)
-        res = (min(lv, pb[nextPower][0]), _smul(s, xs))
+        res = self.mul(self.rescale(*res), pb[nextPower])
         br, tmp = self.recurse(logSplit, tl, cr, pb, res[1])
-        if not _in_delta(tmp[1], res[1], SCALE_PREC - 12):
+        if not self.same_scale(tmp[1], res[1]):
             raise ValueError("recursePS: res.Scale != tmp.Scale")
         return bq + br, res
 
@@ -192,14 +203,14 @@ class _Sym:
     __slots__ = ("slot", "level", "scale", "deg")
 
     def __init__(self, slot, level, scale, deg):
-        self.slot, self.level, self.scale, self.deg = slot, level, Fraction(scale), deg
+        self.slot, self.level, self.scale, self.deg = slot, level, scale, deg
 
 
 class _Lin:
     """A pending linear form sum_k w_k X_k + const (const on component 0): w and const are [limb][half] residues."""
 
     def __init__(self, level, scale, Q):
-        self.level, self.scale, self.Q = level, Fraction(scale), Q[: level + 1]
+        self.level, self.scale, self.Q = level, scale, Q[: level + 1]
         self.w: Dict[int, list] = {}
         self.const = [[0, 0] for _ in self.Q]
 
@@ -442,7 +453,13 @@ class _Planner:
         self.prog.ops.append(dict(kind=TENSOR, dst=y.slot, src0=b.slot, src1=x.slot, addend=a.slot, level=lv, weights=list(rb) + list(ra)))
         return y
 
+    def _sim(self) -> _Sim:
+        return _Sim(self.Q, self.lpr)
+
     def evaluate(self, level, scale, p: _Poly, target_scale) -> Program:
+        """The scheme-independent part of Evaluate (common/polynomial/polynomial_evaluator.go:29-161): level check, power basis,
+        Paterson-Stockmeyer split on the scheme's simEvaluator, every baby step in one LINCOMB, the giant steps, the final
+        Relinearize / Rescale. Scale values are the scheme's (Fractions for CKKS, ints mod t for BGV)."""
         if p.Degree() < 1:
             raise ValueError("the polynomial must have degree >= 1")
         pb: Dict[int, _Sym] = {1: _Sym(0, level, scale, 1)}
@@ -457,12 +474,12 @@ class _Planner:
             if (not (even or odd)) or (i & 1 == 0 and even) or (i & 1 == 1 and odd):
                 self.gen_power(pb, p.Basis, i)
         # PatersonStockmeyerPolynomial with the simulated power basis (polynomial.go:74-106)
-        sim = _Sim(self.Q, self.lpr)
-        spb = {1: (level, Fraction(scale))}
+        sim = self._sim()
+        spb = {1: (level, scale)}
         sim.gen_power(spb, 1 << logDegree)
         for i in range((1 << logSplit) - 1, 2, -1):
             sim.gen_power(spb, i)
-        ps, _ = sim.recurse(logSplit, level - self.lpr * (p.Degree().bit_length() - 1), p, spb, Fraction(target_scale))
+        ps, _ = sim.recurse(logSplit, level - sim.depth(p.Degree()), p, spb, target_scale)
         # every baby step in one LINCOMB
         forms = [self.baby_step(bs, pb, bs.Level, bs.Scale) for bs in ps]
         outs = [_Sym(self._slot(), f.level, f.scale, 1) for f in forms]
