@@ -470,7 +470,9 @@ int lgpu_ckks_special_fft(lgpu_ctx* ctx, double* values, int n, int m, const int
  * Decode: Encoder.DecodePublic (encoder.go:497-762) of `batch` plaintexts pt [level + 1][N]: INTT when LGPU_ENC_NTT (NTT-domain words
  * canonical), then polyToComplexNoCRT (level 0) / polyToComplexCRT, the forward special FFT and, for logprec != 0 (an integer in
  * [-1022, 1023]), math.Round(x 2^logprec) / 2^logprec per part; `values` receives 2^log_slots complex128 per entry (16-byte aligned).
- * With LGPU_ENC_COEFFS: polyToFloatNoCRT / polyToFloatCRT into N float64 per entry, no FFT, logprec unused. Q_level up to 4096 bits. */
+ * With LGPU_ENC_COEFFS: polyToFloatNoCRT / polyToFloatCRT into N float64 per entry, no FFT, logprec unused. At level >= 1 the bit
+ * lengths of q_0..q_level must sum to at most 4096 (the CRT accumulator has 16, 32 or 64 words of 64 bits, chosen from that sum);
+ * past it the call is refused before any launch, even where Q_level itself has fewer than 4096 bits. */
 #define LGPU_ENC_NTT 1
 #define LGPU_ENC_MONTGOMERY 2
 #define LGPU_ENC_COEFFS 4
@@ -620,7 +622,9 @@ int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in,
  * Decode: Decode (encoder.go:471-521) of `batch` plaintexts pt [level + 1][N] (INTT first when LGPU_ENC_NTT; coefficient-domain words may
  * be any 64-bit value): RingQ2T(scaleDown), then MulScalar(scale^-1 mod t); batched: ring-T NTT and the n slots into `values`; with
  * LGPU_ENC_COEFFS: uint64 gives N words, int64 (LGPU_ENC_SIGNED) centres only the first n words and leaves the rest of the entry
- * untouched, as the reference does. Signed words are v - t for v >= t >> 1. Q_level up to 4096 bits. */
+ * untouched, as the reference does. Signed words are v - t for v >= t >> 1. At level > 0 with n < N (gap > 1), the bit lengths of
+ * q_0..q_level must sum to at most 4096 (the CRT accumulator has 16, 32 or 64 words of 64 bits, chosen from that sum); past it the
+ * call is refused before any launch, even where Q_level itself has fewer than 4096 bits. */
 #define LGPU_ENC_SIGNED 8
 #define LGPU_ENC_SCALE_UP 16
 typedef struct lgpu_bgv_encoder lgpu_bgv_encoder;

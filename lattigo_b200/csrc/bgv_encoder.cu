@@ -358,7 +358,7 @@ extern "C" int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int le
     REQUIRE(batch == 1 || (pt_stride >= (size_t)(level + 1) * N && values_stride >= (size_t)tn), "batch strides smaller than one entry");
     const bool big = level > 0 && log_gap > 0;
     const int words = big ? crt_words(c, level) : 0;
-    REQUIRE(words <= kMaxCrtWords, "Q at this level exceeds 4096 bits");
+    REQUIRE(words <= kMaxCrtWords, "the bit lengths of q_0..q_level sum past 4096: the CRT accumulator exceeds 4096 bits");
     REQUIRE_DEVICE(ctx);
     const cudaStream_t st = (cudaStream_t)stream;
     const TMod& T = enc->tm;

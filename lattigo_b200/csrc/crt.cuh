@@ -10,7 +10,7 @@
 
 namespace lgpu {
 
-constexpr int kMaxCrtWords = 64;     // Q_level up to 4096 bits
+constexpr int kMaxCrtWords = 64;     // the bit lengths of q_0..q_level sum to at most 4096 (crt_words)
 
 // Per-call constants of the CRT reconstruction at `level` (host-built): for k <= level, q_k, BRed hi / lo, (Q/q_k)^-1 mod q_k and 1/q_k;
 // then Q/q_k as W words each, Q and floor(Q / 2) as W words.

@@ -290,7 +290,7 @@ extern "C" int lgpu_ckks_decode(lgpu_ctx* ctx, const uint64_t* pt, int level, in
     REQUIRE(values && aligned_to(values, coeffs ? 8 : 16), "null or misaligned values (8-byte float64, 16-byte complex128)");
     REQUIRE(batch == 1 || (pt_stride >= (size_t)(level + 1) * N && values_stride >= (size_t)(coeffs ? N : slots)), "batch strides smaller than one entry");
     const int words = level ? crt_words(c, level) : 0;
-    REQUIRE(words <= kMaxCrtWords, "Q at this level exceeds 4096 bits");
+    REQUIRE(words <= kMaxCrtWords, "the bit lengths of q_0..q_level sum past 4096: the CRT accumulator exceeds 4096 bits");
     REQUIRE_DEVICE(ctx);
     const cudaStream_t st = (cudaStream_t)stream;
     const size_t rows = (size_t)level + 1, poly = rows * N;
