@@ -362,7 +362,20 @@ __global__ void __launch_bounds__(256) mac_kernel(MacParams p) {
         reinterpret_cast<ulonglong2*>(a1)[i] = v1;
     }
 }
-static int launch_mac(const MacParams& p, cudaStream_t st) {
+// the MAC of key digit (i, j); x rows from xa ([batch][nq + xa_pshift + np][N]) except rows [dlo, dhi), read from xb
+static int launch_mac(const Ctx* c, const GadgetCt& evk, int i, int j, const u64* xa, size_t xa_bs, int xa_pshift, CSpan xb, int dlo, int dhi,
+                      const AccSpans& acc, int nq, int np, bool first, bool last, int batch, cudaStream_t st) {
+    const size_t N = c->N;
+    MacParams p;
+    memset(&p, 0, sizeof(p));
+    p.limbs = c->d_limbs; p.evk0 = evk.at(i, j, 0, N); p.evk1 = evk.at(i, j, 1, N); p.nQk = evk.levelQ + 1;
+    p.xa = xa; p.xa_rs = N; p.xa_bs = xa_bs; p.xa_pshift = xa_pshift;
+    p.xb = xb.p; p.xb_rs = xb.row_stride; p.xb_bs = xb.batch_stride;
+    p.dlo = dlo; p.dhi = dhi;
+    for (int k = 0; k < 2; k++) { p.accQ[k] = acc.q[k].p; p.accP[k] = acc.p[k].p; }
+    p.accQ_rs = acc.q[0].row_stride; p.accQ_bs = acc.q[0].batch_stride; p.accP_rs = acc.p[0].row_stride; p.accP_bs = acc.p[0].batch_stride;
+    p.nq = nq; p.np = np; p.nQfull = c->nQ;
+    p.first = first; p.last = last; p.batch = batch; p.n = c->N;
     // algorithmic bytes: evk (2 rows) once + per ciphertext x (1 row) + accumulators (2 rows written, 2 read unless first)
     ProfScope ps(LGPU_KCLASS_MAC, st, 8.0 * p.n * (p.nq + p.np) * (2.0 + p.batch * (p.first ? 3.0 : 5.0)), 1);
     int zb = p.batch < 4 ? p.batch : 4;
@@ -398,21 +411,27 @@ int decompose_single_ntt(const Ctx* c, int levelQ, int levelP, int nbPi, int dig
     return 0;
 }
 
+// Whether the accumulators are one QP-stacked block with uniform strides (rows of N words, each element's P rows right after its nq Q
+// rows, component 1 above component 0), the layout the fused key-switch pipeline takes; blk is that block (ncomp 2).
+static bool stacked_block(const AccSpans& acc, size_t nq, size_t N, Block& blk) {
+    if (!(acc.q[0].row_stride == N && acc.p[0].row_stride == N && acc.p[0].p == acc.q[0].p + nq * N && acc.p[1].p == acc.q[1].p + nq * N &&
+          acc.q[1].p > acc.q[0].p && acc.q[0].batch_stride == acc.q[1].batch_stride && acc.p[0].batch_stride == acc.q[0].batch_stride &&
+          acc.p[1].batch_stride == acc.q[0].batch_stride)) return false;
+    blk = Block{acc.q[0].p, (size_t)(acc.q[1].p - acc.q[0].p), acc.q[0].batch_stride};
+    return true;
+}
+
 // gadgetProductMultiplePLazy, core/rlwe/evaluator_gadget_product.go:129-201 (cx in the NTT domain)
 static int gadget_product_multiple_p_lazy(const Ctx* c, int levelQ, CSpan cx, const GadgetCt& evk, const AccSpans& acc, int batch, cudaStream_t st) {
     const int levelP = evk.levelP;
     const size_t N = c->N, nq = levelQ + 1, np = levelP + 1;
-    // fused pipeline (keyswitch_fused.cu) when the accumulators are QP-stacked blocks with uniform strides
-    if (ks_fused_applicable(c, levelQ, evk) && cx.row_stride == N && acc.q[0].row_stride == N && acc.p[0].row_stride == N &&
-        acc.p[0].p == acc.q[0].p + nq * N && acc.p[1].p == acc.q[1].p + nq * N && acc.q[1].p > acc.q[0].p &&
-        acc.q[0].batch_stride == acc.q[1].batch_stride && acc.p[0].batch_stride == acc.q[0].batch_stride &&
-        acc.p[1].batch_stride == acc.q[0].batch_stride) {
+    Block blk;
+    if (ks_fused_applicable(c, levelQ, evk) && cx.row_stride == N && stacked_block(acc, nq, N, blk)) {
         Scratch inv;
         if (inv.alloc((size_t)batch * nq * N, st)) return -1;
         Span cxInv{inv.p, N, nq * N};
         if (launch_intt(c, rows_range(0, 0, (int)nq), cx, cxInv, batch, NTT_CANONICAL, st)) return -1;
-        return gadget_product_multiple_p_fused(c, levelQ, cx, CSpan{inv.p, N, nq * N}, evk, acc.q[0].p, (size_t)(acc.q[1].p - acc.q[0].p),
-                                               acc.q[0].batch_stride, batch, st);
+        return gadget_product_multiple_p_fused(c, levelQ, cx, CSpan{inv.p, N, nq * N}, evk, blk, batch, st);
     }
     Scratch buf;
     if (buf.alloc((size_t)batch * (nq + nq + np) * N, st)) return -1;
@@ -424,17 +443,8 @@ static int gadget_product_multiple_p_lazy(const Ctx* c, int levelQ, CSpan cx, co
     const int nd = base_rns_decomposition_vector_size(levelQ, levelP);
     for (int i = 0; i < nd; i++) {
         if (decompose_single_ntt(c, levelQ, levelP, levelP + 1, i, cx, CSpan{cxInv.p, N, nq * N}, c2Q, c2P, false, batch, st)) return -1;
-        MacParams m;
-        memset(&m, 0, sizeof(m));
-        m.limbs = c->d_limbs; m.evk0 = evk.at(i, 0, 0, N); m.evk1 = evk.at(i, 0, 1, N); m.nQk = evk.levelQ + 1;
-        m.xa = c2; m.xa_rs = N; m.xa_bs = (nq + np) * N;
-        m.xb = cx.p; m.xb_rs = cx.row_stride; m.xb_bs = cx.batch_stride;
-        m.dlo = i * (levelP + 1); m.dhi = m.dlo + levelP + 1;
-        for (int k = 0; k < 2; k++) { m.accQ[k] = acc.q[k].p; m.accP[k] = acc.p[k].p; }
-        m.accQ_rs = acc.q[0].row_stride; m.accQ_bs = acc.q[0].batch_stride; m.accP_rs = acc.p[0].row_stride; m.accP_bs = acc.p[0].batch_stride;
-        m.nq = (int)nq; m.np = (int)np; m.nQfull = c->nQ;
-        m.first = (i == 0); m.last = (i == nd - 1); m.batch = batch; m.n = c->N;
-        if (launch_mac(m, st)) return -1;
+        if (launch_mac(c, evk, i, 0, c2, (nq + np) * N, 0, cx, i * (levelP + 1), (i + 1) * (levelP + 1), acc, (int)nq, (int)np, i == 0, i == nd - 1,
+                       batch, st)) return -1;
     }
     return 0;
 }
@@ -478,16 +488,8 @@ static int gadget_product_single_p_lazy(const Ctx* c, int levelQ, CSpan cx, cons
                                  0, 0, c->N, st)) return -1;
                 if (launch_ntt(c, rqp, CSpan{c2, N, (nq + np) * N}, Span{c2, N, (nq + np) * N}, batch, NTT_CANONICAL, st)) return -1;
             } else if (launch_ntt(c, rqp, CSpan{c2, N, (nq + np) * N}, Span{c2, N, (nq + np) * N}, batch, NTT_EXACT_LAZY, st)) return -1;
-            MacParams m;
-            memset(&m, 0, sizeof(m));
-            m.limbs = c->d_limbs; m.evk0 = evk.at(i, j, 0, N); m.evk1 = evk.at(i, j, 1, N); m.nQk = evk.levelQ + 1;
-            m.xa = c2; m.xa_rs = N; m.xa_bs = (nq + np) * N;
-            m.xb = nullptr; m.dlo = m.dhi = 0;
-            for (int k = 0; k < 2; k++) { m.accQ[k] = acc.q[k].p; m.accP[k] = acc.p[k].p; }
-            m.accQ_rs = acc.q[0].row_stride; m.accQ_bs = acc.q[0].batch_stride; m.accP_rs = acc.p[0].row_stride; m.accP_bs = acc.p[0].batch_stride;
-            m.nq = (int)nq; m.np = (int)np; m.nQfull = c->nQ;
-            m.first = acc_first && (done == 0); m.last = acc_last && (done == total - 1); m.batch = batch; m.n = c->N;
-            if (launch_mac(m, st)) return -1;
+            if (launch_mac(c, evk, i, j, c2, (nq + np) * N, 0, CSpan{nullptr, 0, 0}, 0, 0, acc, (int)nq, (int)np, acc_first && done == 0,
+                           acc_last && done == total - 1, batch, st)) return -1;
             done++;
         }
     }
@@ -518,20 +520,42 @@ int gadget_product_lazy(const Ctx* c, int levelQ, CSpan cx, const GadgetCt& evk,
     return gadget_product_single_p_lazy(c, levelQ, cx, evk, acc, batch, st);
 }
 
-// Evaluator.ModDown (core/rlwe/evaluator_gadget_product.go:39-97), NTT -> NTT case.
-int evaluator_moddown_ntt(const Ctx* c, int levelQ, int levelP, const AccSpans& acc, Span ct0, Span ct1, int batch, cudaStream_t st) {
-    Span out[2] = {ct0, ct1};
-    {
-        const size_t N = c->N, nq = levelQ + 1;
-        if (levelP >= 0 && fz_applicable(c, levelQ, levelP) && acc.q[0].row_stride == N && acc.p[0].row_stride == N &&
-            acc.p[0].p == acc.q[0].p + nq * N && acc.p[1].p == acc.q[1].p + nq * N && acc.q[1].p > acc.q[0].p &&
-            acc.q[0].batch_stride == acc.q[1].batch_stride && acc.p[0].batch_stride == acc.q[0].batch_stride &&
-            acc.p[1].batch_stride == acc.q[0].batch_stride && ct0.row_stride == N && ct1.row_stride == N && ct1.p > ct0.p &&
-            ct0.batch_stride == ct1.batch_stride && ct0.p != acc.q[0].p) {
-            return moddown_ntt_fused(c, levelQ, levelP, acc.q[0].p, (size_t)(acc.q[1].p - acc.q[0].p), acc.q[0].batch_stride, nullptr, 0, 0,
-                                     ct0.p, (size_t)(ct1.p - ct0.p), ct0.batch_stride, 2, batch, st);
+// Evaluator.ModDown (core/rlwe/evaluator_gadget_product.go:39-97), NTT -> NTT case. The fused pipeline (keyswitch_fused.cu) where it
+// applies; otherwise ModDownQPtoQNTT per component (a copy when levelP = -1), then one Add per component, through a scratch block when
+// the addend is stored in out.
+int moddown_ntt(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock add, Block out, int ncomp, int batch, cudaStream_t st) {
+    if (levelP >= 0 && fz_applicable(c, levelQ, levelP)) return moddown_ntt_fused(c, levelQ, levelP, acc, add, out, ncomp, batch, st);
+    const size_t N = c->N, nq = levelQ + 1;
+    Scratch buf;
+    Block md = out;
+    if (add.p && add.p == out.p) {
+        if (buf.alloc((size_t)ncomp * batch * nq * N, st)) return -1;
+        md = Block{buf.p, (size_t)batch * nq * N, nq * N};
+    }
+    for (int k = 0; k < ncomp; k++) {
+        const u64* a = acc.p + k * acc.cs;
+        u64* o = md.p + k * md.cs;
+        if (levelP != -1) {
+            if (moddown_qp_to_q_ntt(c, levelQ, levelP, CSpan{a, N, acc.bs}, CSpan{a + nq * N, N, acc.bs}, Span{o, N, md.bs}, batch, st)) return -1;
+        } else if (a != o) {
+            LGPU_CUDA_OK(cudaMemcpy2DAsync(o, md.bs * 8, a, acc.bs * 8, nq * N * 8, batch, cudaMemcpyDeviceToDevice, st));
         }
     }
+    if (add.p)
+        for (int k = 0; k < ncomp; k++)
+            if (launch_vecop(c, rows_range(0, 0, (int)nq), LGPU_OP_ADD, CSpan{md.p + k * md.cs, N, md.bs}, CSpan{add.p + k * add.cs, N, add.bs},
+                             Span{out.p + k * out.cs, N, out.bs}, batch, nullptr, nullptr, 0, 0, c->N, st)) return -1;
+    return 0;
+}
+
+// the C-ABI ModDown: any four accumulator spans
+int evaluator_moddown_ntt(const Ctx* c, int levelQ, int levelP, const AccSpans& acc, Span ct0, Span ct1, int batch, cudaStream_t st) {
+    const size_t N = c->N;
+    Block blk;
+    if (stacked_block(acc, levelQ + 1, N, blk) && ct0.row_stride == N && ct1.row_stride == N && ct1.p > ct0.p && ct0.batch_stride == ct1.batch_stride &&
+        ct0.p != acc.q[0].p)
+        return moddown_ntt(c, levelQ, levelP, blk, CBlock{nullptr, 0, 0}, Block{ct0.p, (size_t)(ct1.p - ct0.p), ct0.batch_stride}, 2, batch, st);
+    Span out[2] = {ct0, ct1};
     for (int k = 0; k < 2; k++) {
         CSpan aq{acc.q[k].p, acc.q[k].row_stride, acc.q[k].batch_stride};
         if (levelP != -1) {
@@ -623,16 +647,8 @@ int gadget_product_hoisted_lazy(const Ctx* c, int levelQ, const u64* decomp, con
     const size_t N = c->N, nq = levelQ + 1, np = levelP + 1;
     const int nd = base_rns_decomposition_vector_size(levelQ, levelP);
     for (int i = 0; i < nd; i++) {
-        MacParams m;
-        memset(&m, 0, sizeof(m));
-        m.limbs = c->d_limbs; m.evk0 = evk.at(i, 0, 0, N); m.evk1 = evk.at(i, 0, 1, N); m.nQk = evk.levelQ + 1;
-        m.xa = decomp + (size_t)i * batch * (nqd + np) * N; m.xa_rs = N; m.xa_bs = (nqd + np) * N; m.xa_pshift = (int)(nqd - nq);
-        m.xb = nullptr; m.dlo = m.dhi = 0;
-        for (int k = 0; k < 2; k++) { m.accQ[k] = acc.q[k].p; m.accP[k] = acc.p[k].p; }
-        m.accQ_rs = acc.q[0].row_stride; m.accQ_bs = acc.q[0].batch_stride; m.accP_rs = acc.p[0].row_stride; m.accP_bs = acc.p[0].batch_stride;
-        m.nq = (int)nq; m.np = (int)np; m.nQfull = c->nQ;
-        m.first = (i == 0); m.last = (i == nd - 1); m.batch = batch; m.n = c->N;
-        if (launch_mac(m, st)) return -1;
+        if (launch_mac(c, evk, i, 0, decomp + (size_t)i * batch * (nqd + np) * N, (nqd + np) * N, (int)(nqd - nq), CSpan{nullptr, 0, 0}, 0, 0, acc,
+                       (int)nq, (int)np, i == 0, i == nd - 1, batch, st)) return -1;
     }
     return 0;
 }
@@ -785,23 +801,18 @@ int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_r
     u64* t1 = t0 + (size_t)batch * nq * N;
     if (rlk.levelP >= 1 && rlk.pw2 == 0 && fz_applicable(c, level, rlk.levelP) && (nb_rescales == 0 || (nb_rescales == 1 && level >= 1))) {
         // fused tail: accumulators -> (ModDown + add of d0/d1) in one chunk-pass epilogue -> fused rescale
-        const size_t np = rlk.levelP + 1;
+        const size_t np = rlk.levelP + 1, nqo = nq - nb_rescales;
         Scratch accb;
         if (accb.alloc((size_t)2 * batch * (nq + np) * N, st)) return -1;
         const AccSpans acc = stacked_acc(accb.p, nq, np, N, batch);
         if (gadget_product_lazy(c, level, CSpan{d2, N, nq * N}, rlk, acc, batch, st)) return -1;
-        if (nb_rescales == 1 && moddown_rescale_applicable(c, level)) {
-            const size_t nqo = nq - 1;
-            return moddown_rescale_ntt_fused(c, level, rlk.levelP, accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N, d0, (size_t)batch * nq * N,
-                                             nq * N, out, nqo * N, 2 * nqo * N, 2, batch, st);
-        }
-        // d0, d1 are consecutive [comp][batch][nq][N] blocks: out = d + ModDown(acc), in place
-        if (moddown_ntt_fused(c, level, rlk.levelP, accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N, d0, (size_t)batch * nq * N, nq * N,
-                              d0, (size_t)batch * nq * N, nq * N, 2, batch, st)) return -1;
-        if (nb_rescales == 1) {
-            const size_t nqo = nq - 1;
-            return div_round_last_ntt_fused(c, level, d0, (size_t)batch * nq * N, nq * N, out, nqo * N, 2 * nqo * N, 2, batch, st);
-        }
+        // d0, d1 are consecutive [comp][batch][nq][N] blocks
+        const CBlock ab{accb.p, (size_t)batch * (nq + np) * N, (nq + np) * N};
+        const Block db{d0, (size_t)batch * nq * N, nq * N}, ob{out, nqo * N, 2 * nqo * N};
+        if (nb_rescales == 1 && moddown_rescale_applicable(c, level)) return moddown_rescale_ntt_fused(c, level, rlk.levelP, ab, db, ob, 2, batch, st);
+        // out = d + ModDown(acc), in place
+        if (moddown_ntt(c, level, rlk.levelP, ab, db, db, 2, batch, st)) return -1;
+        if (nb_rescales == 1) return div_round_last_ntt_fused(c, level, db, ob, 2, batch, st);
         for (int k = 0; k < 2; k++)
             LGPU_CUDA_OK(cudaMemcpy2DAsync(out + (size_t)k * nq * N, ct_stride * 8, d0 + (size_t)k * batch * nq * N, nq * N * 8, nq * N * 8, batch,
                                            cudaMemcpyDeviceToDevice, st));

@@ -20,6 +20,16 @@ struct AccSpans {  // the four accumulator polynomials of a ctQP: [comp].Q (leve
     Span q[2];
     Span p[2];
 };
+// ncomp components x batch elements with rows of N words: component k of element b starts at p + k * cs + b * bs
+struct CBlock {
+    const u64* p;
+    size_t cs, bs;
+};
+struct Block {
+    u64* p;
+    size_t cs, bs;
+    operator CBlock() const { return CBlock{p, cs, bs}; }
+};
 struct GaloisKeySet {        // the GaloisKeys map of rlwe.MemEvaluationKeySet, core/rlwe/evaluationkeyset.go
     int n = 0;
     const u64* gal_els = nullptr;
@@ -82,6 +92,9 @@ int decompose_single_ntt(const Ctx* c, int levelQ, int levelP, int nbPi, int dig
 int decompose_ntt(const Ctx* c, int levelQ, int levelP, int nbPi, CSpan c2, bool c2IsNTT, u64* decomp, int batch, cudaStream_t st);
 int gadget_product_lazy(const Ctx* c, int levelQ, CSpan cx, const GadgetCt& evk, const AccSpans& acc, int batch, cudaStream_t st);
 int evaluator_moddown_ntt(const Ctx* c, int levelQ, int levelP, const AccSpans& acc, Span ct0, Span ct1, int batch, cudaStream_t st);
+// out = ModDown(acc) (+ add) for ncomp x batch QP-stacked accumulators (nq Q rows, then the P rows), NTT domain; add.p == nullptr: no
+// addend; add may alias out
+int moddown_ntt(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock add, Block out, int ncomp, int batch, cudaStream_t st);
 int gadget_product(const Ctx* c, int levelQ, CSpan cx, const GadgetCt& evk, Span ct0, Span ct1, int batch, cudaStream_t st);
 int rgsw_external_product(const Ctx* c, const GadgetCt& rg0, const GadgetCt& rg1, CSpan ct0, CSpan ct1, Span out0, Span out1, int batch, cudaStream_t st);
 // decomp_levelQ: level the DecomposeNTT buffer was laid out for (>= levelQ; -1 = levelQ) -- lintrans uses one decomposition for matrices of lower levels
@@ -93,18 +106,14 @@ int evaluator_automorphism(const Ctx* c, int level, CSpan in0, CSpan in1, u64 ga
 int evaluator_relinearize(const Ctx* c, int level, CSpan c0, CSpan c1, CSpan c2, const GadgetCt& rlk, Span out0, Span out1, int batch, cudaStream_t st);
 // keyswitch_fused.cu
 bool ks_fused_applicable(const Ctx* c, int levelQ, const GadgetCt& evk);
-int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cxInv, const GadgetCt& evk, u64* acc, size_t acc_cs, size_t acc_bs,
-                                    int batch, cudaStream_t st);
+int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cxInv, const GadgetCt& evk, Block acc, int batch, cudaStream_t st);
 
 bool fz_applicable(const Ctx* c, int levelQ, int levelP);
-int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs, size_t d_bs,
-                      u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st);
-int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs,
-                             int ncomp, int batch, cudaStream_t st);
+int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock D, Block out, int ncomp, int batch, cudaStream_t st);
+int div_round_last_ntt_fused(const Ctx* c, int level, CBlock X, Block out, int ncomp, int batch, cudaStream_t st);
 // moddown_ntt_fused with addend D followed by div_round_last_ntt_fused (D is overwritten), in fewer passes when Q[levelQ] is an FP64-pipe prime
 bool moddown_rescale_applicable(const Ctx* c, int level);
-int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, u64* D, size_t d_cs,
-                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st);
+int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, Block D, Block out, int ncomp, int batch, cudaStream_t st);
 
 int ckks_mulrelin_rescale(const Ctx* c, int level, const u64* ctA, const u64* ctB, const GadgetCt& rlk, int nb_rescales, u64* out, int batch,
                           cudaStream_t st);

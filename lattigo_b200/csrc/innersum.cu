@@ -50,11 +50,8 @@ __global__ void __launch_bounds__(256) auto_add_kernel(AutoAddParams p) {
 
 namespace {
 
-struct Ct {            // a batch of degree-1 ciphertexts: component k of element b at p + (2b + k) * cs
-    u64* p; size_t cs;
-};
-
-int auto_add(const Ctx* c, int nq, Ct in, const u64* t, int nb, Ct out, u64 galEl, cudaStream_t st) {
+// Every Block below is a batch of degree-1 ciphertexts, [batch][2][.][N]: bs = 2 * cs.
+int auto_add(const Ctx* c, int nq, Block in, const u64* t, int nb, Block out, u64 galEl, cudaStream_t st) {
     if (in.p == out.p) { set_error("auto_add: the output must not alias the input"); return -1; }
     AutoAddParams p;
     int lg = 0;
@@ -68,14 +65,14 @@ int auto_add(const Ctx* c, int nq, Ct in, const u64* t, int nb, Ct out, u64 galE
     return 0;
 }
 
-// rows 0..nq-1 of both components, nb ciphertexts (2 * nb row blocks): NTT / INTT / copy between two Ct layouts
-int ntt_ct(const Ctx* c, bool inverse, int nq, Ct in, Ct out, int nb, cudaStream_t st) {
+// rows 0..nq-1 of both components, nb ciphertexts (2 * nb row blocks): NTT / INTT / copy between two ciphertext layouts
+int ntt_ct(const Ctx* c, bool inverse, int nq, Block in, Block out, int nb, cudaStream_t st) {
     const RowMap rm = rows_range(0, 0, nq);
     const CSpan i{in.p, (size_t)c->N, in.cs};
     const Span o{out.p, (size_t)c->N, out.cs};
     return inverse ? launch_intt(c, rm, i, o, 2 * nb, NTT_CANONICAL, st) : launch_ntt(c, rm, i, o, 2 * nb, NTT_CANONICAL, st);
 }
-int copy_ct(const Ctx* c, int nq, Ct in, Ct out, int nb, cudaStream_t st) {
+int copy_ct(const Ctx* c, int nq, Block in, Block out, int nb, cudaStream_t st) {
     if (in.p == out.p) return 0;
     LGPU_CUDA_OK(cudaMemcpy2DAsync(out.p, out.cs * 8, in.p, in.cs * 8, (size_t)nq * c->N * 8, (size_t)2 * nb, cudaMemcpyDeviceToDevice, st));
     return 0;
@@ -106,8 +103,8 @@ std::vector<u64> trace_elements(const Ctx* c, int log_n) {
     return g;
 }
 
-int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, const std::vector<const GadgetCt*>& lazy_keys,
-              const std::vector<const GadgetCt*>& dbl_keys, Ct out, int nb, cudaStream_t st) {
+int pts_chunk(const Ctx* c, int level, Block in, bool is_ntt, int offset, int n, const std::vector<const GadgetCt*>& lazy_keys,
+              const std::vector<const GadgetCt*>& dbl_keys, Block out, int nb, cudaStream_t st) {
     const int nq = level + 1;
     const size_t N = c->N, ctw = (size_t)2 * nb * nq * N;
     if (n == 1) {
@@ -143,8 +140,8 @@ int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, co
     Scratch buf;
     if (buf.alloc(dec_w + acc_w + c0p_w + ctw /* t */ + nbuf * ctw /* B0, B1 */, st)) return -1;
     u64* decomp = buf.p; u64* accb = decomp + dec_w; u64* c0p = accb + acc_w; u64* t = c0p + c0p_w;
-    const Ct bufs[4] = {out, in, Ct{t + ctw, (size_t)nq * N}, Ct{t + 2 * ctw, (size_t)nq * N}};
-    std::vector<Ct> X(d + 1);
+    const Block bufs[4] = {out, in, Block{t + ctw, (size_t)nq * N, (size_t)2 * nq * N}, Block{t + 2 * ctw, (size_t)nq * N, (size_t)2 * nq * N}};
+    std::vector<Block> X(d + 1);
     for (int s = 0; s <= d; s++) X[s] = bufs[tag[s]];
     if (copy_in && copy_ct(c, nq, in, X[0], nb, st)) return -1;
     if (!is_ntt && ntt_ct(c, false, nq, in, X[0], nb, st)) return -1;
@@ -152,12 +149,12 @@ int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, co
     const std::vector<u64> pq = p_mod_q_mont(c, level, levelP);
     bool first = true;
     for (int i = 0; i < d; i++) {
-        const Ct x = X[i];
+        const Block x = X[i];
         // DecomposeNTT(ctInNTT[1]) once per doubling step; the reference also decomposes in the last iteration, whose result it never reads
-        if (decompose_ntt(c, level, levelP, levelP + 1, CSpan{x.p + x.cs, N, 2 * x.cs}, true, decomp, nb, st)) return -1;
+        if (decompose_ntt(c, level, levelP, levelP + 1, CSpan{x.p + x.cs, N, x.bs}, true, decomp, nb, st)) return -1;
         if (sched[i].lazy) {
             // accQP (+)= AutomorphismHoistedLazy(ctInNTT, k); P * ctInNTT[0] is its Q-row addend (evaluator_automorphism.go:150-156)
-            if (launch_vecop(c, rows_range(0, 0, nq), LGPU_OP_MULSCALARMONTGOMERY, CSpan{x.p, N, 2 * x.cs}, CSpan{nullptr, 0, 0}, Span{c0p, N, (size_t)nq * N},
+            if (launch_vecop(c, rows_range(0, 0, nq), LGPU_OP_MULSCALARMONTGOMERY, CSpan{x.p, N, x.bs}, CSpan{nullptr, 0, 0}, Span{c0p, N, (size_t)nq * N},
                              nb, pq.data(), nullptr, 0, 0, c->N, st)) return -1;
             if (automorphism_hoisted_lazy(c, level, CSpan{c0p, N, (size_t)nq * N}, decomp, level, galois_element(c, sched[i].k), *lazy_keys[i], acc, nb, st, !first))
                 return -1;
@@ -170,24 +167,14 @@ int pts_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int offset, int n, co
     }
     if (n & (n - 1)) {
         // opOut = ModDown(accQP) + ctInNTT (:256-263); X[d] is `out`, so the addend is read and written in place
-        if (fz_applicable(c, level, levelP)) {
-            if (moddown_ntt_fused(c, level, levelP, accb, (size_t)nb * (nq + np) * N, (nq + np) * N, out.p, out.cs, 2 * out.cs, out.p, out.cs, 2 * out.cs, 2,
-                                  nb, st)) return -1;
-        } else {
-            u64* t1 = t + (size_t)nb * nq * N;
-            if (evaluator_moddown_ntt(c, level, levelP, acc, Span{t, N, (size_t)nq * N}, Span{t1, N, (size_t)nq * N}, nb, st)) return -1;
-            for (int k = 0; k < 2; k++)
-                if (launch_vecop(c, rows_range(0, 0, nq), LGPU_OP_ADD, CSpan{t + (size_t)k * nb * nq * N, N, (size_t)nq * N},
-                                 CSpan{out.p + k * out.cs, N, 2 * out.cs}, Span{out.p + k * out.cs, N, 2 * out.cs}, nb, nullptr, nullptr, 0, 0, c->N, st))
-                    return -1;
-        }
+        if (moddown_ntt(c, level, levelP, CBlock{accb, (size_t)nb * (nq + np) * N, (nq + np) * N}, out, out, 2, nb, st)) return -1;
     }
     if (!is_ntt) return ntt_ct(c, true, nq, out, out, nb, st);
     return 0;
 }
 
-int trace_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int log_n, const std::vector<const GadgetCt*>& keys, const std::vector<u64>& els, Ct out,
-                int nb, cudaStream_t st) {
+int trace_chunk(const Ctx* c, int level, Block in, bool is_ntt, int log_n, const std::vector<const GadgetCt*>& keys, const std::vector<u64>& els,
+                Block out, int nb, cudaStream_t st) {
     const int nq = level + 1;
     const size_t N = c->N;
     const int S = (int)els.size();
@@ -195,20 +182,20 @@ int trace_chunk(const Ctx* c, int level, Ct in, bool is_ntt, int log_n, const st
     Scratch buf;
     if (buf.alloc((size_t)4 * nb * nq * N, st)) return -1;
     u64* t = buf.p;
-    const Ct B{buf.p + (size_t)2 * nb * nq * N, (size_t)nq * N};
+    const Block B{buf.p + (size_t)2 * nb * nq * N, (size_t)nq * N, (size_t)2 * nq * N};
     auto X = [&](int s) { return ((S - s) & 1) ? B : out; };    // X_S = out
     // pre-multiplication by gap^-1 mod Q_level (ringQ.MulScalarBigint, canonical per limb), then NTT for a coefficient-domain input
     const int gap_log = c->logN - log_n - 1 + (log_n == 0 ? 1 : 0);
     std::vector<u64> sc(nq);
     for (int i = 0; i < nq; i++) sc[i] = h_mform(h_invmod(((u64)1 << gap_log) % c->Q[i], c->Q[i]), c->Q[i]);
-    const Ct x0 = X(0);
+    const Block x0 = X(0);
     if (launch_vecop(c, rows_range(0, 0, nq), LGPU_OP_MULSCALARMONTGOMERY, CSpan{in.p, N, in.cs}, CSpan{nullptr, 0, 0}, Span{x0.p, N, x0.cs}, 2 * nb, sc.data(),
                      nullptr, 0, 0, c->N, st)) return -1;
     if (!is_ntt && ntt_ct(c, false, nq, x0, x0, nb, st)) return -1;
     for (int s = 1; s <= S; s++) {
-        const Ct x = X(s - 1);
+        const Block x = X(s - 1);
         // opOut += Automorphism(opOut, g) (:85-101)
-        if (gadget_product(c, level, CSpan{x.p + x.cs, N, 2 * x.cs}, *keys[s - 1], Span{t, N, (size_t)nq * N}, Span{t + (size_t)nb * nq * N, N, (size_t)nq * N},
+        if (gadget_product(c, level, CSpan{x.p + x.cs, N, x.bs}, *keys[s - 1], Span{t, N, (size_t)nq * N}, Span{t + (size_t)nb * nq * N, N, (size_t)nq * N},
                            nb, st)) return -1;
         if (auto_add(c, nq, x, t, nb, X(s), els[s - 1], st)) return -1;
     }
@@ -267,7 +254,7 @@ int lgpu_evaluator_partial_traces_sum(lgpu_ctx* ctx, int level, const uint64_t* 
     const int ch = batch_chunk();
     for (int k = 0; k < batch; k += ch) {
         const int nb = std::min(ch, batch - k);
-        const Ct in{(u64*)ct_in + (size_t)k * 2 * cs, cs}, out{(u64*)ct_out + (size_t)k * 2 * cs, cs};
+        const Block in{(u64*)ct_in + (size_t)k * 2 * cs, cs, 2 * cs}, out{(u64*)ct_out + (size_t)k * 2 * cs, cs, 2 * cs};
         if (pts_chunk(&c, level, in, is_ntt != 0, offset, n, lazy_keys, dbl_keys, out, nb, st)) return -1;
     }
     return 0;
@@ -306,7 +293,7 @@ int lgpu_evaluator_trace(lgpu_ctx* ctx, int level_in, const uint64_t* ct_in, int
     const int ch = batch_chunk();
     for (int k = 0; k < batch; k += ch) {
         const int nb = std::min(ch, batch - k);
-        const Ct in{(u64*)ct_in + (size_t)k * 2 * ci, ci}, out{(u64*)ct_out + (size_t)k * 2 * co, co};
+        const Block in{(u64*)ct_in + (size_t)k * 2 * ci, ci, 2 * ci}, out{(u64*)ct_out + (size_t)k * 2 * co, co, 2 * co};
         if (trace_chunk(&c, level, in, is_ntt != 0, log_n, keys, els, out, nb, st)) return -1;
     }
     return 0;

@@ -1093,8 +1093,7 @@ static void split_by_corr(const Ctx* c, const RowMap& in, RowMap& corr, RowMap& 
 
 // acc: QP-stacked accumulators (component c, batch b at acc + c*acc_cs + b*acc_bs, rows 0..nq-1 Q then P; canonical).
 // cx: NTT-domain input, cxInv: its INTT (coefficient domain).
-int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cxInv, const GadgetCt& evk, u64* acc, size_t acc_cs, size_t acc_bs,
-                                    int batch, cudaStream_t st) {
+int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cxInv, const GadgetCt& evk, Block acc, int batch, cudaStream_t st) {
     const int levelP = evk.levelP;
     const int k = levelP + 1, nq = levelQ + 1, np = levelP + 1, nrows = nq + np;
     const int nd = base_rns_decomposition_vector_size(levelQ, levelP);
@@ -1104,11 +1103,10 @@ int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cx
     const size_t y_words = (size_t)batch * nq * N;
     const size_t p1_words = (size_t)batch * nd * nrows * N;
     const size_t v_words = ((size_t)batch * nd * N + 7) / 8;
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, (y_words + p1_words + v_words) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
-    u64* Y = buf;
-    u64* P1 = buf + y_words;
+    Scratch buf;
+    if (buf.alloc(y_words + p1_words + v_words, st)) return -1;
+    u64* Y = buf.p;
+    u64* P1 = buf.p + y_words;
     unsigned char* V = reinterpret_cast<unsigned char*>(P1 + p1_words);
 
     // ---- K1
@@ -1165,7 +1163,7 @@ int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cx
     cp.cx = cx.p; cp.cx_rs = cx.row_stride; cp.cx_bs = cx.batch_stride;
     const size_t key_rows = (size_t)(evk.levelQ + 1) + (size_t)(evk.levelP + 1);
     cp.evk = evk.data; cp.evk_cs = key_rows * N; cp.evk_ds = (size_t)evk.npw2max * 2 * key_rows * N; cp.nQk = evk.levelQ + 1;
-    cp.acc = acc; cp.acc_cs = acc_cs; cp.acc_bs = acc_bs;
+    cp.acc = acc.p; cp.acc_cs = acc.cs; cp.acc_bs = acc.bs;
     cp.logN = c->logN; cp.nq = nq; cp.k = k; cp.nd = nd;
     const size_t smem = (size_t)(4096 + 256 + 8 + 2 * 4096) * sizeof(u64);
     const unsigned gx = (unsigned)(((N >> s1) + 255) / 256);
@@ -1495,8 +1493,8 @@ struct FzModDown {
 };
 
 // A (INTT of the P rows) and B (K1) of the fused ModDown; fills md for fz_moddown_rows
-static int fz_moddown_prepare(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs,
-                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, u64* buf, FzModDown& md, cudaStream_t st) {
+static int fz_moddown_prepare(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock D, Block out, int ncomp, int batch, u64* buf, FzModDown& md,
+                              cudaStream_t st) {
     const int nq = levelQ + 1, np = levelP + 1;
     const size_t N = c->N;
     const int Z = ncomp * batch;
@@ -1508,7 +1506,7 @@ static int fz_moddown_prepare(const Ctx* c, int levelQ, int levelP, const u64* a
     rp.nrows = np;
     for (int j = 0; j < np; j++) { rp.limb[j] = (unsigned char)(c->nQ + j); rp.drow[j] = (unsigned char)j; }
     for (int cc = 0; cc < ncomp; cc++) {
-        CSpan in{acc + (size_t)cc * acc_cs + (size_t)nq * N, N, acc_bs};
+        CSpan in{acc.p + (size_t)cc * acc.cs + (size_t)nq * N, N, acc.bs};
         Span o{buffP + (size_t)cc * batch * np * N, N, (size_t)np * N};
         if (launch_intt(c, rp, in, o, batch, NTT_CANONICAL, st)) return -1;
     }
@@ -1542,8 +1540,8 @@ static int fz_moddown_prepare(const Ctx* c, int levelQ, int levelP, const u64* a
     FzChunkParams& cp = md.cp;
     memset(&cp, 0, sizeof(cp));
     cp.limbs = c->d_limbs; cp.P1 = P1; cp.p1_bs = (size_t)nq * N;
-    cp.A = acc; cp.a_cs = acc_cs; cp.a_bs = acc_bs; cp.D = D; cp.d_cs = d_cs; cp.d_bs = d_bs;
-    cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.nb = batch; cp.logN = c->logN;
+    cp.A = acc.p; cp.a_cs = acc.cs; cp.a_bs = acc.bs; cp.D = D.p; cp.d_cs = D.cs; cp.d_bs = D.bs;
+    cp.out = out.p; cp.o_cs = out.cs; cp.o_bs = out.bs; cp.nb = batch; cp.logN = c->logN;
     return 0;
 }
 
@@ -1581,14 +1579,12 @@ static int fz_moddown_rows(const Ctx* c, int levelP, FzModDown& m, const RowMap&
     return 0;
 }
 
-int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, const u64* D, size_t d_cs, size_t d_bs,
-                      u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st) {
+int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock D, Block out, int ncomp, int batch, cudaStream_t st) {
     const int nq = levelQ + 1;
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, moddown_scratch_words(nq, levelP + 1, ncomp * batch, c->N) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    Scratch buf;
+    if (buf.alloc(moddown_scratch_words(nq, levelP + 1, ncomp * batch, c->N), st)) return -1;
     FzModDown m;
-    if (fz_moddown_prepare(c, levelQ, levelP, acc, acc_cs, acc_bs, D, d_cs, d_bs, out, o_cs, o_bs, ncomp, batch, buf, m, st)) return -1;
+    if (fz_moddown_prepare(c, levelQ, levelP, acc, D, out, ncomp, batch, buf.p, m, st)) return -1;
     RowMap fp, in;
     split_rows(c, 0, nq, fp, in);
     cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
@@ -1605,13 +1601,13 @@ struct FzRescale {
 };
 
 // the INTT r [ncomp][batch][N] of row `level` of X, and the K2 / epilogue parameters of the rescale (P1: [Z] x p1_bs words)
-static int fz_rescale_prepare(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp,
-                              int batch, u64* r, u64* P1, size_t p1_bs, FzRescale& m, cudaStream_t st) {
+static int fz_rescale_prepare(const Ctx* c, int level, CBlock X, Block out, int ncomp, int batch, u64* r, u64* P1, size_t p1_bs, FzRescale& m,
+                              cudaStream_t st) {
     const size_t N = c->N;
     RowMap rl;
     rl.nrows = 1; rl.limb[0] = (unsigned char)level; rl.drow[0] = 0;
     for (int cc = 0; cc < ncomp; cc++) {
-        CSpan in{X + (size_t)cc * x_cs + (size_t)level * N, N, x_bs};
+        CSpan in{X.p + (size_t)cc * X.cs + (size_t)level * N, N, X.bs};
         Span o{r + (size_t)cc * batch * N, N, N};
         if (launch_intt(c, rl, in, o, batch, NTT_CANONICAL, st)) return -1;
     }
@@ -1623,8 +1619,8 @@ static int fz_rescale_prepare(const Ctx* c, int level, const u64* X, size_t x_cs
     FzChunkParams& cp = m.cp;
     memset(&cp, 0, sizeof(cp));
     cp.limbs = c->d_limbs; cp.P1 = P1; cp.p1_bs = p1_bs;
-    cp.A = X; cp.a_cs = x_cs; cp.a_bs = x_bs; cp.D = nullptr;
-    cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.nb = batch; cp.logN = c->logN;
+    cp.A = X.p; cp.a_cs = X.cs; cp.a_bs = X.bs; cp.D = nullptr;
+    cp.out = out.p; cp.o_cs = out.cs; cp.o_bs = out.bs; cp.nb = batch; cp.logN = c->logN;
     return 0;
 }
 
@@ -1663,15 +1659,13 @@ static int fz_rescale_rows(const Ctx* c, int level, FzRescale& m, const RowMap& 
     return 0;
 }
 
-int div_round_last_ntt_fused(const Ctx* c, int level, const u64* X, size_t x_cs, size_t x_bs, u64* out, size_t o_cs, size_t o_bs,
-                             int ncomp, int batch, cudaStream_t st) {
+int div_round_last_ntt_fused(const Ctx* c, int level, CBlock X, Block out, int ncomp, int batch, cudaStream_t st) {
     const size_t N = c->N;
     const int Z = ncomp * batch;
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, ((size_t)Z * N + (size_t)Z * level * N) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
+    Scratch buf;
+    if (buf.alloc((size_t)Z * N + (size_t)Z * level * N, st)) return -1;
     FzRescale m;
-    if (fz_rescale_prepare(c, level, X, x_cs, x_bs, out, o_cs, o_bs, ncomp, batch, buf, buf + (size_t)Z * N, (size_t)level * N, m, st)) return -1;
+    if (fz_rescale_prepare(c, level, X, out, ncomp, batch, buf.p, buf.p + (size_t)Z * N, (size_t)level * N, m, st)) return -1;
     RowMap fp, in;
     split_rows(c, 0, level, fp, in);
     cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
@@ -1694,19 +1688,17 @@ bool moddown_rescale_applicable(const Ctx* c, int level) {
 //     out_i = (X_i - NTT(e_i)) q_L^-1 = (acc_i - NTT(m_i + [P]_{q_i} e_i)) (P q_L)^-1 + D_i q_L^-1,
 // with m_i the ModDown's basis extension and e_i the rescale's broadcast value of INTT(X_L), both computed as in the two stages: the
 // canonical outputs are the same. D keeps its FP64 rows below L.
-int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* acc, size_t acc_cs, size_t acc_bs, u64* D, size_t d_cs,
-                              size_t d_bs, u64* out, size_t o_cs, size_t o_bs, int ncomp, int batch, cudaStream_t st) {
+int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, Block D, Block out, int ncomp, int batch, cudaStream_t st) {
     const int nq = levelQ + 1, np = levelP + 1, L = levelQ;
     const size_t N = c->N;
     const int Z = ncomp * batch;
     const int s1 = c->logN - 12;
     const size_t md_words = moddown_scratch_words(nq, np, Z, N);
-    u64* buf = nullptr;
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&buf, (md_words + (size_t)Z * N) * sizeof(u64), st));
-    struct Free { u64* p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); } } guard{buf, st};
-    u64* r = buf + md_words;
+    Scratch buf;
+    if (buf.alloc(md_words + (size_t)Z * N, st)) return -1;
+    u64* r = buf.p + md_words;
     FzModDown md;
-    if (fz_moddown_prepare(c, levelQ, levelP, acc, acc_cs, acc_bs, D, d_cs, d_bs, D, d_cs, d_bs, ncomp, batch, buf, md, st)) return -1;
+    if (fz_moddown_prepare(c, levelQ, levelP, acc, D, D, ncomp, batch, buf.p, md, st)) return -1;
     RowMap fp, in, last, none;
     split_rows(c, 0, L, fp, in);
     last.nrows = 1; last.limb[0] = last.drow[0] = (unsigned char)L;
@@ -1717,7 +1709,7 @@ int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* a
     join_side(c, st, sint);
     // INTT of X_L; the rescale of the integer rows (the ModDown's P1 rows are free again)
     FzRescale rs;
-    if (fz_rescale_prepare(c, L, D, d_cs, d_bs, out, o_cs, o_bs, ncomp, batch, r, md.sp.P1, (size_t)nq * N, rs, st)) return -1;
+    if (fz_rescale_prepare(c, L, D, out, ncomp, batch, r, md.sp.P1, (size_t)nq * N, rs, st)) return -1;
     sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
     if (fz_rescale_rows(c, L, rs, none, in, ncomp, batch, st, sint)) return -1;
     // the FP64 rows below L: one K2 and one epilogue
@@ -1725,7 +1717,7 @@ int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, const u64* a
         KsStridedParams& sp = md.sp;
         sp.rm = fp; sp.bc = r; sp.bc_bs = N; sp.bc_add = rs.sp.bc_add; sp.bc_q = rs.sp.bc_q;
         FzChunkParams cp = md.cp;
-        cp.rm = fp; cp.out = out; cp.o_cs = o_cs; cp.o_bs = o_bs; cp.dscale = 1;
+        cp.rm = fp; cp.out = out.p; cp.o_cs = out.cs; cp.o_bs = out.bs; cp.dscale = 1;
         const u64 qL = c->Q[L];
         for (int k = 0; k < fp.nrows; k++) {
             const u64 qi = c->Q[fp.drow[k]];

@@ -239,11 +239,7 @@ void bsgs_index(const LinTransView& m, std::map<int, std::vector<int>>& index, s
 
 namespace {
 
-struct Buf {   // owned scratch block, freed on the stream
-    u64* p = nullptr; cudaStream_t st = nullptr;
-    ~Buf() { if (p) cudaFreeAsync(p, st); }
-};
-typedef std::map<int, std::unique_ptr<Buf>> PreRot;   // baby step -> [comp][batch][nqd + np][N]
+typedef std::map<int, std::unique_ptr<Scratch>> PreRot;   // baby step -> [comp][batch][nqd + np][N]
 
 struct LtState {
     const Ctx* c; cudaStream_t st; int batch;
@@ -289,9 +285,8 @@ static int prerotate(const LtState& s, const std::vector<int>& rots, PreRot& pre
         const GadgetCt* gk = s.gks->find(galEl);
         if (!gk) return -1;
         if (check_key_level_p(s.levelP, galEl, *gk)) return -1;
-        std::unique_ptr<Buf> b(new Buf);
-        b->st = s.st;
-        LGPU_CUDA_OK(cudaMallocAsync((void**)&b->p, per * sizeof(u64), s.st));
+        std::unique_ptr<Scratch> b(new Scratch);
+        if (b->alloc(per, s.st)) return -1;
         AccSpans out = stacked_acc(b->p, s.nqd, s.np, s.N, s.batch);
         if (automorphism_hoisted_lazy(s.c, s.levelQd, CSpan{s.ctP, s.N, s.nqd * s.N}, s.decomp, s.levelQd, galEl, *gk, out, s.batch, s.st)) return -1;
         pre[i] = std::move(b);
@@ -407,9 +402,7 @@ static int multiply_bsgs(const LtState& s, const LinTransView& m, const PreRot& 
         if (j != 0) {
             // hoisted ModDown of the c1 part, key-switch to the giant-step rotation, rotate, accumulate (:409-436)
             u64* t1 = tb + per / 2;
-            if (fz_applicable(c, levelQ, s.levelP)) {
-                if (moddown_ntt_fused(c, levelQ, s.levelP, t1, 0, sbs, nullptr, 0, 0, t1d, 0, nq * N, 1, s.batch, s.st)) return -1;
-            } else if (moddown_qp_to_q_ntt(c, levelQ, s.levelP, CSpan{t1, N, sbs}, CSpan{t1 + nq * N, N, sbs}, Span{t1d, N, nq * N}, s.batch, s.st)) return -1;
+            if (moddown_ntt(c, levelQ, s.levelP, CBlock{t1, 0, sbs}, CBlock{nullptr, 0, 0}, Block{t1d, 0, nq * N}, 1, s.batch, s.st)) return -1;
             const u64 galEl = galois_element(c, j);
             const GadgetCt* gk = s.gks->find(galEl);
             if (!gk) return -1;

@@ -128,30 +128,25 @@ int keyswitch_c1(const Ctx* c, int level, bool ntt, CSpan c1, const GadgetCt& ke
     return 0;
 }
 
-// same-degree applyEvaluationKey (:99-107) on nb ciphertexts: out = (c0 + ks0, ks1). `in` and `out` may be the same block (the
-// key switch reads all of c1 before writing, the addition is element-wise).
-int apply_same(const Ctx* c, int level, bool ntt, const u64* in, size_t in_cs, u64* out, size_t out_cs, const GadgetCt& key, u64* ks, u64* t,
-               int nb, cudaStream_t st) {
+// same-degree applyEvaluationKey (:99-107) on nb ciphertexts ([batch][2][level + 1][N] blocks): out = (c0 + ks0, ks1). `in` and `out` may be
+// the same block (the key switch reads all of c1 before writing, the addition is element-wise).
+int apply_same(const Ctx* c, int level, bool ntt, CBlock in, Block out, const GadgetCt& key, u64* ks, u64* t, int nb, cudaStream_t st) {
     const size_t N = c->N, cs = (size_t)(level + 1) * N;
-    const RowMap rm = rows_range(0, 0, level + 1);
-    if (ntt && key.levelP >= 0 && fz_applicable(c, level, key.levelP)) {
-        // fused ModDown epilogue, one call per component: out[0] = ModDown(acc[0]) + c0 (the addend folded in), out[1] = ModDown(acc[1])
+    if (ntt) {
+        // one ModDown per component: out[0] = ModDown(acc[0]) + c0, out[1] = ModDown(acc[1]); the fused ModDown adds c0 in its epilogue
         const size_t nq = level + 1, np = key.levelP + 1, qp = (nq + np) * N;
         Scratch acc_buf;
         if (acc_buf.alloc((size_t)2 * nb * qp, st)) return -1;
         const AccSpans acc = stacked_acc(acc_buf.p, nq, np, N, nb);
-        if (gadget_product_lazy(c, level, CSpan{in + in_cs, N, 2 * in_cs}, key, acc, nb, st)) return -1;
-        if (moddown_ntt_fused(c, level, key.levelP, acc_buf.p, 0, qp, in, 0, 2 * in_cs, out, 0, 2 * out_cs, 1, nb, st)) return -1;
-        return moddown_ntt_fused(c, level, key.levelP, acc_buf.p + (size_t)nb * qp, 0, qp, nullptr, 0, 0, out + out_cs, 0, 2 * out_cs, 1, nb, st);
+        if (gadget_product_lazy(c, level, CSpan{in.p + in.cs, N, in.bs}, key, acc, nb, st)) return -1;
+        if (moddown_ntt(c, level, key.levelP, CBlock{acc_buf.p, 0, qp}, CBlock{in.p, 0, in.bs}, Block{out.p, 0, out.bs}, 1, nb, st)) return -1;
+        return moddown_ntt(c, level, key.levelP, CBlock{acc_buf.p + (size_t)nb * qp, 0, qp}, CBlock{nullptr, 0, 0}, Block{out.p + out.cs, 0, out.bs}, 1,
+                           nb, st);
     }
-    if (ntt) {
-        // ks1 goes straight to out[1]
-        if (gadget_product(c, level, CSpan{in + in_cs, N, 2 * in_cs}, key, Span{ks, N, cs}, Span{out + out_cs, N, 2 * out_cs}, nb, st)) return -1;
-    } else {
-        if (keyswitch_c1(c, level, false, CSpan{in + in_cs, N, 2 * in_cs}, key, ks, t, nb, st)) return -1;
-        LGPU_CUDA_OK(cudaMemcpy2DAsync(out + out_cs, 2 * out_cs * 8, ks + (size_t)nb * cs, cs * 8, cs * 8, nb, cudaMemcpyDeviceToDevice, st));
-    }
-    return launch_vecop(c, rm, LGPU_OP_ADD, CSpan{in, N, 2 * in_cs}, CSpan{ks, N, cs}, Span{out, N, 2 * out_cs}, nb, nullptr, nullptr, 0, 0, c->N, st);
+    if (keyswitch_c1(c, level, false, CSpan{in.p + in.cs, N, in.bs}, key, ks, t, nb, st)) return -1;
+    LGPU_CUDA_OK(cudaMemcpy2DAsync(out.p + out.cs, out.bs * 8, ks + (size_t)nb * cs, cs * 8, cs * 8, nb, cudaMemcpyDeviceToDevice, st));
+    return launch_vecop(c, rows_range(0, 0, level + 1), LGPU_OP_ADD, CSpan{in.p, N, in.bs}, CSpan{ks, N, cs}, Span{out.p, N, out.bs}, nb, nullptr,
+                        nullptr, 0, 0, c->N, st);
 }
 
 int apply_run(const Ctx* c, const u64* in, int n_in, int level_in, bool ntt, const GadgetCt& key, u64* out, int n_out, int level_out, int B,
@@ -183,15 +178,16 @@ int apply_run(const Ctx* c, const u64* in, int n_in, int level_in, bool ntt, con
         LGPU_CUDA_OK(cudaGetLastError());
         for (int e0 = 0; e0 < B; e0 += ch) {
             const int nb = std::min(ch, B - e0);
-            u64* o = out + (size_t)e0 * 2 * out_cs;
-            if (apply_same(c, level, ntt, o, out_cs, o, out_cs, key, ks, t, nb, st)) return -1;
+            const Block o{out + (size_t)e0 * 2 * out_cs, out_cs, 2 * out_cs};
+            if (apply_same(c, level, ntt, o, o, key, ks, t, nb, st)) return -1;
         }
         return 0;
     }
     if (n_in == n_out) {
         for (int e0 = 0; e0 < B; e0 += ch) {
             const int nb = std::min(ch, B - e0);
-            if (apply_same(c, level, ntt, in + (size_t)e0 * 2 * in_cs, in_cs, out + (size_t)e0 * 2 * out_cs, out_cs, key, ks, t, nb, st)) return -1;
+            if (apply_same(c, level, ntt, CBlock{in + (size_t)e0 * 2 * in_cs, in_cs, 2 * in_cs}, Block{out + (size_t)e0 * 2 * out_cs, out_cs, 2 * out_cs}, key,
+                           ks, t, nb, st)) return -1;
         }
         return 0;
     }
