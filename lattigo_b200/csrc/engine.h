@@ -53,6 +53,16 @@ struct RowMap {
     unsigned char drow[kMaxRows];  // data row (within the polynomial) of launch row r
 };
 
+// Splits the rows of `rm` into those whose global limb satisfies `pred` and the others, in their order within each class.
+template <class Pred>
+inline void partition_rows(const RowMap& rm, Pred pred, RowMap& yes, RowMap& no) {
+    yes.nrows = no.nrows = 0;
+    for (int r = 0; r < rm.nrows; r++) {
+        RowMap& d = pred(rm.limb[r]) ? yes : no;
+        d.limb[d.nrows] = rm.limb[r]; d.drow[d.nrows] = rm.drow[r]; d.nrows++;
+    }
+}
+
 struct HostSubRing {
     u64 q, qinv, bred_hi, bred_lo, ninv, primitive_root;
     std::vector<u64> roots_fwd, roots_bwd;  // host copies (also returned through the C ABI for cross-checks)
@@ -159,7 +169,7 @@ struct CSpan {
     size_t batch_stride;
 };
 
-enum NttMode { NTT_CANONICAL = 0, NTT_EXACT_LAZY = 1, NTT_REFERENCE_ARITH = 2 };
+enum NttMode { NTT_CANONICAL = 0, NTT_EXACT_LAZY = 1 };
 
 int launch_ntt(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st);
 int launch_intt(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st);
@@ -169,6 +179,12 @@ int launch_vecop(const Ctx* c, const RowMap& rm, int op, CSpan p1, CSpan p2, Spa
 
 // ntt_fp64.cu
 bool fp64_ntt_supported(const Ctx* c);
+// whether the transforms of global limb `limb` run on the FP64 pipe
+inline bool on_fp64_pipe(const Ctx* c, int limb) { return c->h_limbs[limb].fp_ok && fp64_ntt_supported(c); }
+// the rows of `rm` that run on the FP64 pipe, and the integer rows
+inline void split_fp64_rows(const Ctx* c, const RowMap& rm, RowMap& fp, RowMap& rest) {
+    partition_rows(rm, [c](int limb) { return on_fp64_pipe(c, limb); }, fp, rest);
+}
 // conjugate-invariant ring (ntt_ci.cu); lazy selects NTTConjugateInvariantLazy / INTTConjugateInvariantLazy
 int launch_ntt_ci(const Ctx* c, const RowMap& rm, bool inverse, CSpan in, Span out, int batch, int lazy, cudaStream_t st);
 int launch_ntt_fp64(const Ctx* c, const RowMap& rm, bool inverse, CSpan in, Span out, int batch, cudaStream_t st);

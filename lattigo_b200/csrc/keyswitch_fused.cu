@@ -1084,11 +1084,7 @@ static int ks_launch_strided(int rl, int nsmax, const KsStridedParams& p, dim3 g
 // integer rows whose prime needs the lazy-correction schedule (fwd_mask != 0: above 2^57) vs rows that never correct: the second class
 // runs instantiations with the correction compiled out
 static void split_by_corr(const Ctx* c, const RowMap& in, RowMap& corr, RowMap& plain) {
-    corr.nrows = plain.nrows = 0;
-    for (int r = 0; r < in.nrows; r++) {
-        RowMap& d = c->h_limbs[in.limb[r]].fwd_mask != 0 ? corr : plain;
-        d.limb[d.nrows] = in.limb[r]; d.drow[d.nrows] = in.drow[r]; d.nrows++;
-    }
+    partition_rows(in, [c](int limb) { return c->h_limbs[limb].fwd_mask != 0; }, corr, plain);
 }
 
 // acc: QP-stacked accumulators (component c, batch b at acc + c*acc_cs + b*acc_bs, rows 0..nq-1 Q then P; canonical).
@@ -1147,12 +1143,7 @@ int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cx
     }
     // row classes
     RowMap fp, in;
-    fp.nrows = in.nrows = 0;
-    for (int r = 0; r < nrows; r++) {
-        const int limb = r < nq ? r : c->nQ + (r - nq);
-        RowMap& dst = (c->h_limbs[limb].fp_ok && fp64_ntt_supported(c)) ? fp : in;
-        dst.limb[dst.nrows] = (unsigned char)limb; dst.drow[dst.nrows] = (unsigned char)r; dst.nrows++;
-    }
+    split_fp64_rows(c, rows_qp(c, nq, np), fp, in);
     // ---- K2 + K3: FP64 rows on `st`, integer rows on the side stream
     sp.limbs = c->d_limbs; sp.blob = c->d_blob; sp.Y = Y; sp.y_bs = (size_t)nq * N; sp.V = V; sp.v_bs = (size_t)nd * N;
     sp.P1 = P1; sp.p1_ds = (size_t)nrows * N; sp.p1_bs = (size_t)nd * nrows * N;
@@ -1464,15 +1455,6 @@ static int fz_launch_chunk(const FzChunkParams& p, dim3 grid, cudaStream_t st) {
     return 0;
 }
 
-static void split_rows(const Ctx* c, int limb0, int nrows, RowMap& fp, RowMap& in) {
-    fp.nrows = in.nrows = 0;
-    for (int r = 0; r < nrows; r++) {
-        const int limb = limb0 + r;
-        RowMap& dst = (c->h_limbs[limb].fp_ok && fp64_ntt_supported(c)) ? fp : in;
-        dst.limb[dst.nrows] = (unsigned char)limb; dst.drow[dst.nrows] = (unsigned char)r; dst.nrows++;
-    }
-}
-
 bool fz_applicable(const Ctx* c, int levelQ, int levelP) {
     static const int off = [] { const char* e = getenv("LGPU_NO_FUSED_KS"); return e && atoi(e) ? 1 : 0; }();
     if (off || c->ring_type != 0 || c->logN < 13 || c->logN > 16) return false;
@@ -1586,7 +1568,7 @@ int moddown_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, CBlock D
     FzModDown m;
     if (fz_moddown_prepare(c, levelQ, levelP, acc, D, out, ncomp, batch, buf.p, m, st)) return -1;
     RowMap fp, in;
-    split_rows(c, 0, nq, fp, in);
+    split_fp64_rows(c, rows_range(0, 0, nq), fp, in);
     cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
     if (fz_moddown_rows(c, levelP, m, fp, in, ncomp, batch, st, sint)) return -1;
     join_side(c, st, sint);
@@ -1667,7 +1649,7 @@ int div_round_last_ntt_fused(const Ctx* c, int level, CBlock X, Block out, int n
     FzRescale m;
     if (fz_rescale_prepare(c, level, X, out, ncomp, batch, buf.p, buf.p + (size_t)Z * N, (size_t)level * N, m, st)) return -1;
     RowMap fp, in;
-    split_rows(c, 0, level, fp, in);
+    split_fp64_rows(c, rows_range(0, 0, level), fp, in);
     cudaStream_t sint = fork_side(c, st, fp.nrows > 0 && in.nrows > 0);
     if (fz_rescale_rows(c, level, m, fp, in, ncomp, batch, st, sint)) return -1;
     join_side(c, st, sint);
@@ -1678,7 +1660,7 @@ int div_round_last_ntt_fused(const Ctx* c, int level, CBlock X, Block out, int n
 // row-sharing kernel only, so LGPU_K2_J4=0 selects the two stages too.
 bool moddown_rescale_applicable(const Ctx* c, int level) {
     static const int on = [] { const char* e = getenv("LGPU_FUSED_RESCALE"); return e ? atoi(e) : 1; }();
-    return on && k2_j4() && level >= 1 && c->h_limbs[level].fp_ok && fp64_ntt_supported(c);
+    return on && k2_j4() && level >= 1 && on_fp64_pipe(c, level);
 }
 
 // ModDown with an addend, then the rescale by q_L = Q[levelQ], for ncomp x batch QP-stacked accumulators, when q_L is an FP64-pipe prime:
@@ -1700,7 +1682,7 @@ int moddown_rescale_ntt_fused(const Ctx* c, int levelQ, int levelP, CBlock acc, 
     FzModDown md;
     if (fz_moddown_prepare(c, levelQ, levelP, acc, D, D, ncomp, batch, buf.p, md, st)) return -1;
     RowMap fp, in, last, none;
-    split_rows(c, 0, L, fp, in);
+    split_fp64_rows(c, rows_range(0, 0, L), fp, in);
     last.nrows = 1; last.limb[0] = last.drow[0] = (unsigned char)L;
     none.nrows = 0;
     // the ModDown on row L and the integer rows

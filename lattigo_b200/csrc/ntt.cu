@@ -13,7 +13,7 @@
 // the launch's working set fits in the 50 MB L2), once when logN <= 12.
 //
 // Arithmetic, two variants selected at compile time (template parameter FAST):
-//   FAST = false : the reference's lazy Montgomery butterflies (ring/ntt.go:155-171) with the reference's own
+//   FAST = false : forward only: the reference's lazy Montgomery butterflies (ring/ntt.go:155-171) with the reference's own
 //                  4q-correction schedule, so NTT_EXACT_LAZY reproduces NTTLazy's representative in [0, 6q)
 //                  bit for bit (used only when a caller asks for the Lazy API).
 //   FAST = true  : free-form path for canonical outputs (NTT / INTT / INTTLazy for N >= 16): Shoup products with
@@ -46,6 +46,7 @@ struct NttParams {
 // ---------------------------------------------------------------------------------------------------
 template <int RL, bool INVERSE, int FAST>
 __global__ void __launch_bounds__(256) ntt_strided_kernel(NttParams p) {
+    static_assert(!INVERSE || FAST != 0, "the inverse transform has fast kernels only");
     constexpr int R = 1 << RL;
     const int b = blockIdx.z;
     const LimbConst L = p.limbs[p.rm.limb[blockIdx.y]];
@@ -87,21 +88,6 @@ __global__ void __launch_bounds__(256) ntt_strided_kernel(NttParams p) {
                 fast_fwd_bfly(x[k], x[k + half], w, nq, twoq, L.kq, corr);
             }
         }
-    } else if constexpr (INVERSE && !FAST) {
-        const u64* roots = L.roots_bwd;
-#pragma unroll
-        for (int u = RL - 1; u >= 0; u--) {
-            const int half = 1 << (RL - 1 - u);
-#pragma unroll
-            for (int k = 0; k < R; k++) {
-                if (k & half) continue;
-                u64 tw = __ldg(roots + (1 << u) + (k >> (RL - u)));
-                inv_bfly(x[k], x[k + half], tw, q, qinv);
-            }
-        }
-        // x N^-1 (Montgomery), canonical: ring/ntt.go:185-206 (mulscalarmontgomeryvec, also for the Lazy API when N >= 16)
-#pragma unroll
-        for (int k = 0; k < R; k++) x[k] = mred(x[k], L.ninv, q, qinv);
     } else {
         const ulonglong2* tw = L.tw_bwd;
         const bool lazy = (FAST == 2) || (FAST == 1 && L.inv_lazy != 0);
@@ -188,6 +174,7 @@ ntt_chunk_fwd_kernel(NttParams p) {
 template <int CL, int FAST>
 __global__ void __launch_bounds__((1 << CL) >= 16 ? ((1 << CL) / 16) : 1)
 ntt_chunk_inv_kernel(NttParams p) {
+    static_assert(FAST != 0, "the inverse transform has fast kernels only");
     constexpr int C = 1 << CL;
     constexpr int T = C / 16;
     constexpr int NR = num_rounds(CL);
@@ -221,43 +208,39 @@ ntt_chunk_inv_kernel(NttParams p) {
 // ---------------------------------------------------------------------------------------------------
 // host launchers
 // ---------------------------------------------------------------------------------------------------
-template <int CL>
-static int launch_chunk(bool inverse, int fast, const NttParams& p, dim3 grid, cudaStream_t st) {
+template <bool INV, int FAST, int CL>
+static void launch_chunk(const NttParams& p, dim3 grid, cudaStream_t st) {
     constexpr int C = 1 << CL;
     constexpr int T = C >= 16 ? C / 16 : 1;
-    size_t smem = (size_t)(C + (C >> 4) + 1) * sizeof(u64);
-    if (inverse) {
-        if (fast == 2) ntt_chunk_inv_kernel<CL, 2><<<grid, T, smem, st>>>(p);
-        else if (fast == 1) ntt_chunk_inv_kernel<CL, 1><<<grid, T, smem, st>>>(p);
-        else ntt_chunk_inv_kernel<CL, 0><<<grid, T, smem, st>>>(p);
+    const size_t smem = (size_t)(C + (C >> 4) + 1) * sizeof(u64);
+    if constexpr (INV) {
+        ntt_chunk_inv_kernel<CL, FAST><<<grid, T, smem, st>>>(p);
+    } else if constexpr (FAST == 2 && CL == 12) {
+        static const int minb = [] { const char* e = getenv("LGPU_NTT_MINB"); return e ? atoi(e) : 2; }();
+        if (minb == 3) ntt_chunk_fwd_kernel<CL, 2, 3><<<grid, T, smem, st>>>(p);
+        else if (minb == 4) ntt_chunk_fwd_kernel<CL, 2, 4><<<grid, T, smem, st>>>(p);
+        else ntt_chunk_fwd_kernel<CL, 2, 2><<<grid, T, smem, st>>>(p);
     } else {
-        if (fast == 2) {
-            static const int minb = [] { const char* e = getenv("LGPU_NTT_MINB"); return e ? atoi(e) : 2; }();
-            if (CL == 12 && minb == 3) ntt_chunk_fwd_kernel<CL, 2, (CL == 12 ? 3 : 1)><<<grid, T, smem, st>>>(p);
-            else if (CL == 12 && minb == 4) ntt_chunk_fwd_kernel<CL, 2, (CL == 12 ? 4 : 1)><<<grid, T, smem, st>>>(p);
-            else ntt_chunk_fwd_kernel<CL, 2, (CL == 12 ? 2 : 1)><<<grid, T, smem, st>>>(p);
-        }
-        else if (fast == 1) ntt_chunk_fwd_kernel<CL, 1><<<grid, T, smem, st>>>(p);
-        else ntt_chunk_fwd_kernel<CL, 0><<<grid, T, smem, st>>>(p);
+        ntt_chunk_fwd_kernel<CL, FAST><<<grid, T, smem, st>>>(p);
+    }
+}
+
+template <bool INV, int FAST>
+static int launch_chunk_dyn(int cl, const NttParams& p, dim3 grid, cudaStream_t st) {
+    switch (cl) {
+        case 4: launch_chunk<INV, FAST, 4>(p, grid, st); break;
+        case 5: launch_chunk<INV, FAST, 5>(p, grid, st); break;
+        case 6: launch_chunk<INV, FAST, 6>(p, grid, st); break;
+        case 7: launch_chunk<INV, FAST, 7>(p, grid, st); break;
+        case 8: launch_chunk<INV, FAST, 8>(p, grid, st); break;
+        case 9: launch_chunk<INV, FAST, 9>(p, grid, st); break;
+        case 10: launch_chunk<INV, FAST, 10>(p, grid, st); break;
+        case 11: launch_chunk<INV, FAST, 11>(p, grid, st); break;
+        case 12: launch_chunk<INV, FAST, 12>(p, grid, st); break;
+        default: set_error("unsupported chunk size"); return -1;
     }
     LGPU_CUDA_OK(cudaGetLastError());
     return 0;
-}
-
-static int launch_chunk_dyn(int cl, bool inverse, int fast, const NttParams& p, dim3 grid, cudaStream_t st) {
-    switch (cl) {
-        case 4: return launch_chunk<4>(inverse, fast, p, grid, st);
-        case 5: return launch_chunk<5>(inverse, fast, p, grid, st);
-        case 6: return launch_chunk<6>(inverse, fast, p, grid, st);
-        case 7: return launch_chunk<7>(inverse, fast, p, grid, st);
-        case 8: return launch_chunk<8>(inverse, fast, p, grid, st);
-        case 9: return launch_chunk<9>(inverse, fast, p, grid, st);
-        case 10: return launch_chunk<10>(inverse, fast, p, grid, st);
-        case 11: return launch_chunk<11>(inverse, fast, p, grid, st);
-        case 12: return launch_chunk<12>(inverse, fast, p, grid, st);
-    }
-    set_error("unsupported chunk size");
-    return -1;
 }
 
 template <bool INV, int FAST>
@@ -278,16 +261,30 @@ static int launch_strided(int rl, const NttParams& p, int rows, int batch, cudaS
     return 0;
 }
 
-// the tile queue pays a fill / drain of ~D limb-transforms. H100, one 44-limb polynomial (44 limb-transforms): forward 1.57 vs 1.87 us per
-// limb-transform on the 45-bit chain but 1.78 vs 1.76 on 61-bit primes, inverse 1.71 vs 1.66 and 1.86 vs 1.78 (profiles/h100_ntt_ab.json),
-// so launches below 64 limb-transforms keep the two-pass kernels
-static bool persist_worthwhile(int limb_transforms) {
-    static const int forced = [] { const char* e = getenv("LGPU_NTT_PERSIST"); return e ? atoi(e) : -1; }();
-    return forced == 1 || limb_transforms >= 64;
+// the two-pass integer transform: forward strided pass then chunk pass, inverse chunk pass then strided pass (in place on `out`)
+template <bool INV, int FAST>
+static int launch_int_two_pass(const Ctx* c, const RowMap& rm, int mode, CSpan in, Span out, int batch, cudaStream_t st) {
+    NttParams p;
+    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
+    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
+    p.logN = c->logN; p.mode = mode; p.ci = 0;
+    const int cl = c->logN > 12 ? 12 : c->logN;
+    const int s1 = c->logN - cl;
+    const dim3 grid(1u << s1, rm.nrows, batch);
+    if constexpr (INV) {
+        if (launch_chunk_dyn<true, FAST>(cl, p, grid, st)) return -1;
+        if (s1 == 0) return 0;
+        p.in = out.p; p.in_rs = out.row_stride; p.in_bs = out.batch_stride;
+        return launch_strided<true, FAST>(s1, p, rm.nrows, batch, st);
+    } else {
+        if (s1 > 0 && launch_strided<false, FAST>(s1, p, rm.nrows, batch, st)) return -1;
+        return launch_chunk_dyn<false, FAST>(cl, p, grid, st);
+    }
 }
 
-// 2 = every limb of the launch needs no lazy correction at all (forward: fwd_mask == 0; inverse: inv_lazy), so the
-// correction code is compiled out; 1 = per-limb schedules evaluated at run time.
+// fast: 2 = every limb of the launch needs no lazy correction at all (forward: fwd_mask == 0; inverse: inv_lazy), so the
+// correction code is compiled out; 1 = per-limb schedules evaluated at run time; 0 = the reference's Montgomery arithmetic
+// (forward NTT_EXACT_LAZY only: INTTLazy == INTT for N >= 16, ring/ntt.go:197-206, so both inverse modes are canonical).
 static int fast_variant(const Ctx* c, const RowMap& rm, bool inverse) {
     for (int r = 0; r < rm.nrows; r++) {
         const LimbConst& L = c->h_limbs[rm.limb[r]];
@@ -296,133 +293,95 @@ static int fast_variant(const Ctx* c, const RowMap& rm, bool inverse) {
     return 2;
 }
 
+static int launch_int_two_pass(const Ctx* c, const RowMap& rm, bool inverse, int fast, int mode, CSpan in, Span out, int batch,
+                               cudaStream_t st) {
+    if (inverse) return fast == 2 ? launch_int_two_pass<true, 2>(c, rm, mode, in, out, batch, st)
+                                  : launch_int_two_pass<true, 1>(c, rm, mode, in, out, batch, st);
+    return fast == 2 ? launch_int_two_pass<false, 2>(c, rm, mode, in, out, batch, st)
+         : fast == 1 ? launch_int_two_pass<false, 1>(c, rm, mode, in, out, batch, st)
+                     : launch_int_two_pass<false, 0>(c, rm, mode, in, out, batch, st);
+}
+
+// LGPU_NTT_PERSIST: 0 = never, 1 = every canonical transform the persistent kernels serve, unset = launches of at least 64
+// limb-transforms. H100 (700 W), N = 2^16 x 44 limbs x 16 polynomials, us per limb-transform persistent vs two-pass
+// (profiles/h100_ntt_ab.json): forward 0.71 vs 1.14 (45-bit chain) and 1.05 vs 1.27 (61-bit primes), inverse 0.76 vs 0.99 and
+// 1.17 vs 1.24. But the tile queue pays a fill / drain of ~D limb-transforms: one 44-limb polynomial (44 limb-transforms), forward
+// 1.57 vs 1.87 us per limb-transform on the 45-bit chain but 1.78 vs 1.76 on 61-bit primes, inverse 1.71 vs 1.66 and 1.86 vs
+// 1.78, so launches below 64 limb-transforms keep the two-pass kernels.
+static bool persistent(const Ctx* c, int limb_transforms) {
+    static const int forced = [] { const char* e = getenv("LGPU_NTT_PERSIST"); return e ? atoi(e) : -1; }();
+    return forced != 0 && ntt_persist_supported(c) && (forced == 1 || limb_transforms >= 64);
+}
+
+// one row class of a transform: the FP64-pipe rows (fp64) or the integer rows (their fast_variant), persistent or two-pass;
+// mul: the product fused into a persistent forward FP64 launch
+static int launch_rows(const Ctx* c, const RowMap& rm, bool inverse, bool fp64, int fast, bool persist, int mode, CSpan in, Span out,
+                       int batch, CSpan mul, cudaStream_t st) {
+    ProfScope ps(inverse ? LGPU_KCLASS_NTT_INV : LGPU_KCLASS_NTT_FWD, st, (mul.p ? 24.0 : 16.0) * c->N * rm.nrows * batch,
+                 persist ? 1 : (c->logN > 12 ? 2 : 1));
+    if (persist) return launch_ntt_persist(c, rm, inverse, fp64 ? 0 : fast, in, out, batch, st, mul);
+    if (fp64) return launch_ntt_fp64(c, rm, inverse, in, out, batch, st);
+    return launch_int_two_pass(c, rm, inverse, fast, mode, in, out, batch, st);
+}
+
+// out = out * mul (MulCoeffsMontgomery) on the rows of rm; nothing when there is no multiplicand
+static int mul_coeffs(const Ctx* c, const RowMap& rm, CSpan mul, Span out, int batch, cudaStream_t st) {
+    if (!mul.p || rm.nrows == 0) return 0;
+    return launch_vecop(c, rm, LGPU_OP_MULCOEFFSMONTGOMERY, CSpan{out.p, out.row_stride, out.batch_stride}, mul, out, batch, nullptr, nullptr, 0, 0,
+                        c->N, st);
+}
+
 static int check_common(const Ctx* c, const RowMap& rm, int batch) {
     if (c->logN < 4 || c->logN > 17) { set_error("NTT requires 16 <= N <= 2^17"); return -1; }
     if (rm.nrows <= 0 || rm.nrows > kMaxRows || batch <= 0 || batch > 65535) { set_error("bad rows/batch"); return -1; }
     return 0;
 }
 
-// canonical transforms: rows whose prime qualifies go to the FP64-pipe kernels, the rest to the integer kernels
-static bool split_rows_fp64(const Ctx* c, const RowMap& rm, RowMap& fp, RowMap& rest) {
-    fp.nrows = rest.nrows = 0;
-    if (!fp64_ntt_supported(c)) return false;
-    for (int r = 0; r < rm.nrows; r++) {
-        RowMap& d = c->h_limbs[rm.limb[r]].fp_ok ? fp : rest;
-        d.limb[d.nrows] = rm.limb[r]; d.drow[d.nrows] = rm.drow[r]; d.nrows++;
+// Every transform's kernels, chosen per row class; mul.p: Ring.NTT followed by Ring.MulCoeffsMontgomery(., mul, out).
+//   inverse (both modes): each class goes persistent on its own size;
+//   forward, NTT_EXACT_LAZY: the integer Montgomery kernels (FAST = 0) on every row, never persistent;
+//   forward, canonical: the FP64 rows go persistent on the size of the whole launch, the integer rows on their own size. The
+//     two-pass FP64 forward chunk pass stores 128 bits at a time (the persistent kernels use 64-bit accesses only), so without the
+//     persistent kernels an output that is not 16-byte aligned with even strides sends every row to the integer kernels.
+//   The product (SURVEY 8(d) C2(ii): 3 rows of traffic instead of the 5 of the two-call sequence) is fused into a persistent FP64
+//     launch; the integer rows are bound by the integer pipes, which the product would share, so they and every row of a launch
+//     that is not persistent take the coefficient-wise kernel after their transform.
+static int transform(const Ctx* c, const RowMap& rm, bool inverse, int mode, CSpan in, Span out, int batch, CSpan mul, cudaStream_t st) {
+    if (check_common(c, rm, batch)) return -1;
+    if (c->ring_type != 0) {
+        if (launch_ntt_ci(c, rm, inverse, in, out, batch, mode == NTT_EXACT_LAZY, st)) return -1;
+        return mul_coeffs(c, rm, mul, out, batch, st);
     }
-    return fp.nrows > 0;
+    RowMap fp, rest;
+    split_fp64_rows(c, rm, fp, rest);
+    if (inverse) {
+        if (fp.nrows && launch_rows(c, fp, true, true, 0, persistent(c, fp.nrows * batch), mode, in, out, batch, {}, st)) return -1;
+        if (rest.nrows == 0) return 0;
+        return launch_rows(c, rest, true, false, fast_variant(c, rest, true), persistent(c, rest.nrows * batch), mode, in, out, batch, {}, st);
+    }
+    if (mode == NTT_EXACT_LAZY) return launch_rows(c, rm, false, false, 0, false, mode, in, out, batch, {}, st);
+    const bool whole = persistent(c, rm.nrows * batch);
+    if (!whole && !(aligned16(out.p) && even_words(out.row_stride, out.batch_stride))) { fp.nrows = 0; rest = rm; }
+    if (fp.nrows && launch_rows(c, fp, false, true, 0, whole, mode, in, out, batch, whole ? mul : CSpan{}, st)) return -1;
+    if (rest.nrows &&
+        launch_rows(c, rest, false, false, fast_variant(c, rest, false), persistent(c, rest.nrows * batch), mode, in, out, batch, {}, st))
+        return -1;
+    return mul_coeffs(c, whole ? rest : rm, mul, out, batch, st);
 }
-
-static int launch_ntt_int(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st);
-static int launch_intt_int(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st);
 
 int launch_ntt(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st) {
-    if (check_common(c, rm, batch)) return -1;
-    if (c->ring_type != 0) return launch_ntt_ci(c, rm, false, in, out, batch, mode == NTT_EXACT_LAZY, st);
-    RowMap fp, rest;
-    const bool persist = mode == NTT_CANONICAL && ntt_persist_supported(c) && persist_worthwhile(rm.nrows * batch);
-    // the two-pass FP64 forward chunk pass stores 128 bits at a time; the persistent kernels use 64-bit accesses only
-    const bool vec_ok = persist || (aligned16(out.p) && even_words(out.row_stride, out.batch_stride));
-    if (mode == NTT_CANONICAL && vec_ok && split_rows_fp64(c, rm, fp, rest)) {
-        {
-            ProfScope ps(LGPU_KCLASS_NTT_FWD, st, 16.0 * c->N * fp.nrows * batch, persist ? 1 : (c->logN > 12 ? 2 : 1));
-            if (persist ? launch_ntt_persist(c, fp, false, 0, in, out, batch, st) : launch_ntt_fp64(c, fp, false, in, out, batch, st)) return -1;
-        }
-        if (rest.nrows == 0) return 0;
-        return launch_ntt_int(c, rest, in, out, batch, mode, st);
-    }
-    return launch_ntt_int(c, rm, in, out, batch, mode, st);
+    return transform(c, rm, false, mode, in, out, batch, {}, st);
 }
 
-// Ring.NTT + Ring.MulCoeffsMontgomery in one pass (SURVEY 8(d) C2(ii)): algorithmic traffic 3 rows (in, other, out) instead of the
-// 5 of the two-call sequence.
+int launch_intt(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st) {
+    return transform(c, rm, true, mode, in, out, batch, {}, st);
+}
+
 int launch_ntt_mul_montgomery(const Ctx* c, const RowMap& rm, CSpan in, CSpan other, Span out, int batch, cudaStream_t st) {
     if (check_common(c, rm, batch)) return -1;
     if (!other.p) { set_error("null operand"); return -1; }
     if (other.p == out.p) { set_error("NTT+MulCoeffsMontgomery: the multiplicand cannot be the output"); return -1; }
-    if (c->ring_type == 0 && ntt_persist_supported(c) && persist_worthwhile(rm.nrows * batch)) {
-        RowMap fp, rest;
-        if (!split_rows_fp64(c, rm, fp, rest)) { rest = rm; fp.nrows = 0; }
-        if (fp.nrows > 0) {
-            ProfScope ps(LGPU_KCLASS_NTT_FWD, st, 24.0 * c->N * fp.nrows * batch, 1);
-            if (launch_ntt_persist(c, fp, false, 0, in, out, batch, st, other)) return -1;
-        }
-        // integer rows: their transform is bound by the integer pipes, which the product would share, so they keep the transform
-        // followed by the coefficient-wise kernel
-        if (rest.nrows > 0) {
-            if (launch_ntt_int(c, rest, in, out, batch, NTT_CANONICAL, st)) return -1;
-            return launch_vecop(c, rest, LGPU_OP_MULCOEFFSMONTGOMERY, CSpan{out.p, out.row_stride, out.batch_stride}, other, out, batch, nullptr, nullptr, 0, 0,
-                                c->N, st);
-        }
-        return 0;
-    }
-    if (launch_ntt(c, rm, in, out, batch, NTT_CANONICAL, st)) return -1;
-    return launch_vecop(c, rm, LGPU_OP_MULCOEFFSMONTGOMERY, CSpan{out.p, out.row_stride, out.batch_stride}, other, out, batch, nullptr, nullptr, 0, 0, c->N, st);
-}
-
-int launch_intt(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st) {
-    if (check_common(c, rm, batch)) return -1;
-    if (c->ring_type != 0) return launch_ntt_ci(c, rm, true, in, out, batch, mode == NTT_EXACT_LAZY, st);
-    RowMap fp, rest;
-    if (mode != NTT_REFERENCE_ARITH && split_rows_fp64(c, rm, fp, rest)) {
-        {
-            const bool persist = ntt_persist_supported(c) && persist_worthwhile(fp.nrows * batch);
-            ProfScope ps(LGPU_KCLASS_NTT_INV, st, 16.0 * c->N * fp.nrows * batch, persist ? 1 : (c->logN > 12 ? 2 : 1));
-            if (persist ? launch_ntt_persist(c, fp, true, 0, in, out, batch, st) : launch_ntt_fp64(c, fp, true, in, out, batch, st)) return -1;
-        }
-        if (rest.nrows == 0) return 0;
-        return launch_intt_int(c, rest, in, out, batch, mode, st);
-    }
-    return launch_intt_int(c, rm, in, out, batch, mode, st);
-}
-
-static int launch_ntt_int(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st) {
-    if (check_common(c, rm, batch)) return -1;
-    NttParams p;
-    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
-    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
-    p.logN = c->logN; p.mode = mode; p.ci = 0;
-    const int cl = c->logN > 12 ? 12 : c->logN;
-    const int s1 = c->logN - cl;
-    const int fast = (mode == NTT_CANONICAL) ? fast_variant(c, rm, false) : 0;
-    const bool persist = fast != 0 && ntt_persist_supported(c) && persist_worthwhile(rm.nrows * batch);
-    ProfScope ps(LGPU_KCLASS_NTT_FWD, st, 16.0 * c->N * rm.nrows * batch, (s1 > 0 && !persist) ? 2 : 1);
-    if (persist) return launch_ntt_persist(c, rm, false, fast, in, out, batch, st);
-    if (s1 > 0) {
-        int rc = fast == 2 ? launch_strided<false, 2>(s1, p, rm.nrows, batch, st)
-               : fast == 1 ? launch_strided<false, 1>(s1, p, rm.nrows, batch, st)
-                           : launch_strided<false, 0>(s1, p, rm.nrows, batch, st);
-        if (rc) return -1;
-    }
-    dim3 grid(1u << s1, rm.nrows, batch);
-    return launch_chunk_dyn(cl, false, fast, p, grid, st);
-}
-
-static int launch_intt_int(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, int mode, cudaStream_t st) {
-    // INTTLazy == INTT for N >= 16 (ring/ntt.go:197-206): both are canonical, so both take the fast path;
-    // NTT_REFERENCE_ARITH keeps the Montgomery kernels reachable (cross-check in the tests).
-    const int fast = (mode != NTT_REFERENCE_ARITH) ? fast_variant(c, rm, true) : 0;
-    if (check_common(c, rm, batch)) return -1;
-    NttParams p;
-    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
-    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
-    p.logN = c->logN; p.mode = mode; p.ci = 0;
-    const int cl = c->logN > 12 ? 12 : c->logN;
-    const int s1 = c->logN - cl;
-    const bool persist = fast != 0 && ntt_persist_supported(c) && persist_worthwhile(rm.nrows * batch);
-    ProfScope ps(LGPU_KCLASS_NTT_INV, st, 16.0 * c->N * rm.nrows * batch, (s1 > 0 && !persist) ? 2 : 1);
-    if (persist) return launch_ntt_persist(c, rm, true, fast, in, out, batch, st);
-    dim3 grid(1u << s1, rm.nrows, batch);
-    if (launch_chunk_dyn(cl, true, fast, p, grid, st)) return -1;
-    if (s1 > 0) {
-        // second pass works in place on `out`
-        NttParams p2 = p;
-        p2.in = out.p; p2.in_rs = out.row_stride; p2.in_bs = out.batch_stride;
-        return fast == 2 ? launch_strided<true, 2>(s1, p2, rm.nrows, batch, st)
-             : fast == 1 ? launch_strided<true, 1>(s1, p2, rm.nrows, batch, st)
-                         : launch_strided<true, 0>(s1, p2, rm.nrows, batch, st);
-    }
-    return 0;
+    return transform(c, rm, false, NTT_CANONICAL, in, out, batch, other, st);
 }
 
 }  // namespace lgpu

@@ -286,8 +286,8 @@ __device__ __forceinline__ void fp_fwd_round_tw_out(const double* sm, const doub
 template <int CL, int A, int RB, bool TO_GLOBAL, bool SCALE, int FAST>
 __device__ __forceinline__ void inv_round(u64* sm, u64* gdst, const LimbConst& L,
                                           int s1, int chunk, int tid) {
-    const u64 q = L.q, qinv = L.qinv, ninv = L.ninv;
-    const u64* roots = L.roots_bwd;
+    static_assert(FAST != 0, "the inverse transform has fast kernels only");
+    const u64 q = L.q;
     const ulonglong2* twp = L.tw_bwd;
     const bool lazy = L.inv_lazy != 0;
     constexpr int G = 16 >> RB;
@@ -306,43 +306,34 @@ __device__ __forceinline__ void inv_round(u64* sm, u64* gdst, const LimbConst& L
             const int half = 1 << (RB - 1 - u);
             const int s = s1 + A + u;
             const int twbase = (1 << s) + (chunk << (A + u)) + (hi << u);
-            if constexpr (FAST) {
-                // `done` inverse stages precede this one; lazy inputs are < 2^(done+1) q
-                const int done = (CL - 1) - (A + u);
-                if (SCALE && A + u == 0) {
-                    // very last stage of a single-pass transform: fold N^-1, canonical outputs
-                    const u64 addq = lazy ? (q << (done + 1)) : (q << 1);
-#pragma unroll
-                    for (int k = 0; k < RR; k++) {
-                        if (k & half) continue;
-                        const u64 U = x[k], V = x[k + half];
-                        const u64 a = shoup_mul(U + V, L.ninv_s, q);
-                        const u64 c = shoup_mul(U - V + addq, L.last_inv_s, q);
-                        x[k] = a >= q ? a - q : a;
-                        x[k + half] = c >= q ? c - q : c;
-                    }
-                } else {
-                    const u64 addq = lazy ? (q << (done + 1)) : (q << 1);
-#pragma unroll
-                    for (int k = 0; k < RR; k++) {
-                        if (k & half) continue;
-                        const ulonglong2 w = __ldg(twp + twbase + (k >> (RB - u)));
-                        fast_inv_bfly(x[k], x[k + half], w, q, addq, !lazy);
-                    }
-                }
-            } else {
+            // `done` inverse stages precede this one; lazy inputs are < 2^(done+1) q
+            const int done = (CL - 1) - (A + u);
+            if (SCALE && A + u == 0) {
+                // very last stage of a single-pass transform: fold N^-1, canonical outputs
+                const u64 addq = lazy ? (q << (done + 1)) : (q << 1);
 #pragma unroll
                 for (int k = 0; k < RR; k++) {
                     if (k & half) continue;
-                    u64 tw = __ldg(roots + twbase + (k >> (RB - u)));
-                    inv_bfly(x[k], x[k + half], tw, q, qinv);
+                    const u64 U = x[k], V = x[k + half];
+                    const u64 a = shoup_mul(U + V, L.ninv_s, q);
+                    const u64 c = shoup_mul(U - V + addq, L.last_inv_s, q);
+                    x[k] = a >= q ? a - q : a;
+                    x[k + half] = c >= q ? c - q : c;
+                }
+            } else {
+                const u64 addq = lazy ? (q << (done + 1)) : (q << 1);
+#pragma unroll
+                for (int k = 0; k < RR; k++) {
+                    if (k & half) continue;
+                    const ulonglong2 w = __ldg(twp + twbase + (k >> (RB - u)));
+                    fast_inv_bfly(x[k], x[k + half], w, q, addq, !lazy);
                 }
             }
         }
 #pragma unroll
         for (int k = 0; k < RR; k++) {
             const int idx = base + (k << LOB);
-            if (TO_GLOBAL) gdst[idx] = (SCALE && FAST == 0) ? mred(x[k], ninv, q, qinv) : x[k];
+            if (TO_GLOBAL) gdst[idx] = x[k];
             else sm[pad_idx(idx)] = x[k];
         }
     }

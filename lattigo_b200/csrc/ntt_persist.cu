@@ -862,49 +862,6 @@ __global__ void __launch_bounds__(512, 2) ntt_persist_tma_kernel(PersistParams p
     }
 }
 
-template <int RL>
-static int persist_launch_tma(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, cudaStream_t st, CSpan mul) {
-    using Ops = FpFwdOps2<RL>;
-    static int occ = 0, sms = 0;
-    constexpr size_t smem = 2 * 4096 * sizeof(u64);
-    auto kern = ntt_persist_tma_kernel<RL>;
-    if (occ == 0) {
-        LGPU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int o = 0;
-        LGPU_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kern, Ops::T, smem));
-        cudaDeviceProp prop;
-        LGPU_CUDA_OK(cudaGetDeviceProperties(&prop, c->device));
-        sms = prop.multiProcessorCount;
-        occ = o > 0 ? o : 1;
-    }
-    PersistParams p;
-    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
-    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
-    p.logN = c->logN; p.batch = batch; p.nLT = rm.nrows * batch;
-    p.mul = mul.p; p.mul_rs = mul.row_stride; p.mul_bs = mul.batch_stride;
-    p.n1 = Ops::kN1; p.n2 = Ops::kN2;
-    const int per = p.n1 + p.n2;
-    const long tiles = (long)p.nLT * per;
-    int grid = sms * occ;
-    if ((long)grid > tiles) grid = (int)tiles;
-    static const int dmul = [] { const char* e = getenv("LGPU_NTT_PERSIST_D"); return e ? atoi(e) : 0; }();
-    int D = dmul > 0 ? dmul : (int)((5L * grid / 2 + per - 1) / per);
-    if (D < 1) D = 1;
-    p.D = D;
-    p.total = (p.nLT + D) * per;
-    unsigned* ctr = nullptr;
-    const size_t bytes = (size_t)(1 + p.nLT) * sizeof(unsigned);
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&ctr, bytes, st));
-    LGPU_CUDA_OK(cudaMemsetAsync(ctr, 0, bytes, st));
-    p.ctr = ctr;
-    const int tma_ok = aligned16(out.p) && even_words(out.row_stride, out.batch_stride) ? 1 : 0;
-    kern<<<grid, Ops::T, smem, st>>>(p, tma_ok);
-    cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ctr, st);
-    if (e != cudaSuccess) { set_error(std::string("ntt_persist_tma_kernel: ") + cudaGetErrorString(e)); return -1; }
-    return 0;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // Fourth-generation loop (LGPU_NTT_PERSIST_V=6, A/B), forward FP64 with the register copy-out: STATIC tile schedule (tile t belongs to CTA t mod grid;
 // every CTA of the persistent grid is resident and walks its tiles in increasing order, and a pass-2 tile only ever waits for tiles with smaller
@@ -941,140 +898,119 @@ __global__ void __launch_bounds__(Ops::T, Ops::MINB) ntt_persist3_kernel(Persist
     }
 }
 
-template <class Ops>
-static int persist_launch3(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, cudaStream_t st, CSpan mul) {
-    static int occ = 0, sms = 0;
-    auto kern = ntt_persist3_kernel<Ops>;
-    const size_t smem = 2 * Ops::kSmem;
-    if (occ == 0) {
-        LGPU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int o = 0;
-        LGPU_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kern, Ops::T, smem));
-        cudaDeviceProp prop;
-        LGPU_CUDA_OK(cudaGetDeviceProperties(&prop, c->device));
-        sms = prop.multiProcessorCount;
-        occ = o > 0 ? o : 1;
-    }
-    PersistParams p;
-    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
-    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
-    p.logN = c->logN; p.batch = batch; p.nLT = rm.nrows * batch;
-    p.mul = mul.p; p.mul_rs = mul.row_stride; p.mul_bs = mul.batch_stride;
-    p.n1 = Ops::kN1; p.n2 = Ops::kN2;
-    const int per = p.n1 + p.n2;
-    const long tiles = (long)p.nLT * per;
-    int grid = sms * occ;                       // never more than the resident CTAs: the static schedule relies on it
-    if ((long)grid > tiles) grid = (int)tiles;
-    static const int dmul = [] { const char* e = getenv("LGPU_NTT_PERSIST_D"); return e ? atoi(e) : 0; }();
-    int D = dmul > 0 ? dmul : (int)((5L * grid / 2 + per - 1) / per);
-    if (D < 1) D = 1;
-    p.D = D;
-    p.total = (p.nLT + D) * per;
-    unsigned* ctr = nullptr;
-    const size_t bytes = (size_t)(1 + p.nLT) * sizeof(unsigned);
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&ctr, bytes, st));
-    LGPU_CUDA_OK(cudaMemsetAsync(ctr, 0, bytes, st));
-    p.ctr = ctr;
-    kern<<<grid, Ops::T, smem, st>>>(p);
-    cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ctr, st);
-    if (e != cudaSuccess) { set_error(std::string("ntt_persist3_kernel: ") + cudaGetErrorString(e)); return -1; }
-    return 0;
+// ---------------------------------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------------------------------
+static int env_int(const char* name, int dflt) {
+    const char* e = getenv(name);
+    return e ? atoi(e) : dflt;
 }
 
-template <class Ops, bool LOOP2 = false>
-static int persist_launch(const Ctx* c, const RowMap& rm, CSpan in, Span out, int batch, cudaStream_t st, CSpan mul) {
-    static int occ = 0, sms = 0;
-    auto kern = LOOP2 ? ntt_persist2_kernel<Ops> : ntt_persist_kernel<Ops>;
-    if (occ == 0) {
-        LGPU_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Ops::kSmem));
-        int o = 0;
-        LGPU_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kern, Ops::T, Ops::kSmem));
-        cudaDeviceProp prop;
-        LGPU_CUDA_OK(cudaGetDeviceProperties(&prop, c->device));
-        sms = prop.multiProcessorCount;
-        occ = o > 0 ? o : 1;
-    }
-    PersistParams p;
-    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
-    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
-    p.logN = c->logN; p.batch = batch; p.nLT = rm.nrows * batch;
-    p.mul = mul.p; p.mul_rs = mul.row_stride; p.mul_bs = mul.batch_stride;
+// The development switches of the persistent kernels, read once per process.
+//   v: 1 = first generation (padded tile, CTA barriers, serial ticket), 2 = first-generation tile code under the claim-ahead loop,
+//      3 (default) = swizzled tile + pair/warp syncs + claim-ahead loop, 4 = 3 + TMA bulk prefetch of the next chunk (no faster than
+//      3 on the H100: 0.73 vs 0.71 us per limb-transform, profiles/h100_ntt_ab.json), 5 = 3 with the register copy-out (FpFwdOps3),
+//      6 = 5 under the static-schedule / double-buffered loop
+//   iv: integer forward tile code, 3 (default) = 512 x 8 swizzled (IntFwdOps2), 2 = 256 x 16 padded (IntFwdOps)
+//   ph1int: FpFwdOps with an integer first pass
+//   d: the distance D, > 0 overrides the default
+struct PersistSwitches {
+    int v, iv, ph1int, d;
+};
+static const PersistSwitches& switches() {
+    static const PersistSwitches s = {env_int("LGPU_NTT_PERSIST_V", 3), env_int("LGPU_NTT_PERSIST_IV", 3), env_int("LGPU_NTT_PH1INT", 0),
+                                      env_int("LGPU_NTT_PERSIST_D", 0)};
+    return s;
+}
+
+struct Occupancy {
+    int blocks;        // resident CTAs per SM, at least 1
+    cudaError_t err;
+};
+template <class K>
+static Occupancy occupancy(K kern, int threads, size_t smem) {
+    Occupancy o = {0, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)};
+    if (o.err == cudaSuccess) o.err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o.blocks, kern, threads, smem);
+    if (o.blocks < 1) o.blocks = 1;
+    return o;
+}
+
+// One launch of the persistent loop KERN running the tile code Ops, p filled but for the tiles, the distance and the counters. The
+// grid is every resident CTA (SMs x occupancy; the static schedule relies on never having more), clamped to the number of tiles.
+template <class Ops, auto KERN, class... Extra>
+static int persist_launch(const char* name, size_t smem, const Ctx* c, PersistParams p, cudaStream_t st, Extra... extra) {
+    static const Occupancy occ = occupancy(KERN, Ops::T, smem);
+    if (occ.err != cudaSuccess) { set_error(std::string(name) + ": " + cudaGetErrorString(occ.err)); return -1; }
     p.n1 = Ops::kN1; p.n2 = Ops::kN2;
     const int per = p.n1 + p.n2;
     const long tiles = (long)p.nLT * per;
-    int grid = sms * occ;
+    int grid = c->sms * occ.blocks;
     if ((long)grid > tiles) grid = (int)tiles;
-    static const int dmul = [] { const char* e = getenv("LGPU_NTT_PERSIST_D"); return e ? atoi(e) : 0; }();
     // distance: the pass-1 tiles of a step must have left the machine when its pass-2 tiles are drawn, i.e. D steps should
     // hold ~2.5x the resident CTAs
-    int D = dmul > 0 ? dmul : (int)((5L * grid / 2 + per - 1) / per);
+    int D = switches().d > 0 ? switches().d : (int)((5L * grid / 2 + per - 1) / per);
     if (D < 1) D = 1;
     p.D = D;
     p.total = (p.nLT + D) * per;
-    unsigned* ctr = nullptr;
     const size_t bytes = (size_t)(1 + p.nLT) * sizeof(unsigned);
-    LGPU_CUDA_OK(cudaMallocAsync((void**)&ctr, bytes, st));
-    LGPU_CUDA_OK(cudaMemsetAsync(ctr, 0, bytes, st));
-    p.ctr = ctr;
-    kern<<<grid, Ops::T, Ops::kSmem, st>>>(p);
+    LGPU_CUDA_OK(cudaMallocAsync((void**)&p.ctr, bytes, st));
+    LGPU_CUDA_OK(cudaMemsetAsync(p.ctr, 0, bytes, st));
+    KERN<<<grid, Ops::T, smem, st>>>(p, extra...);
     cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ctr, st);
-    if (e != cudaSuccess) { set_error(std::string("ntt_persist_kernel: ") + cudaGetErrorString(e)); return -1; }
+    cudaFreeAsync(p.ctr, st);
+    if (e != cudaSuccess) { set_error(std::string(name) + ": " + cudaGetErrorString(e)); return -1; }
     return 0;
 }
 
-// LGPU_NTT_PERSIST: 0 = never, 1 = every canonical transform, unset = launches of at least 64 limb-transforms (persist_worthwhile,
-// ntt.cu). H100 (700 W), N = 2^16 x 44 limbs x 16 polynomials, us per limb-transform persistent vs two-pass (profiles/h100_ntt_ab.json):
-// forward 0.71 vs 1.14 (45-bit chain) and 1.05 vs 1.27 (61-bit primes), inverse 0.76 vs 0.99 and 1.17 vs 1.24.
+// the first-generation loop (v = 1) or the claim-ahead loop (v >= 2)
+template <class Ops>
+static int ticket_loop(const Ctx* c, const PersistParams& p, cudaStream_t st, bool claim_ahead) {
+    if (claim_ahead) return persist_launch<Ops, ntt_persist2_kernel<Ops>>("ntt_persist2_kernel", Ops::kSmem, c, p, st);
+    return persist_launch<Ops, ntt_persist_kernel<Ops>>("ntt_persist_kernel", Ops::kSmem, c, p, st);
+}
+
+// vec: the output (and the multiplicand, if any) takes 128-bit accesses
+template <int RL>
+static int persist_dispatch(const Ctx* c, const PersistParams& p, bool inverse, int kind, bool vec, bool vec_out, cudaStream_t st) {
+    const PersistSwitches& sw = switches();
+    if (kind == 0) {
+        if (inverse) return ticket_loop<FpInvOps<RL>>(c, p, st, sw.v >= 2);
+        if (sw.ph1int) return ticket_loop<FpFwdOps<RL, 1>>(c, p, st, false);
+        if (sw.v == 4)
+            return persist_launch<FpFwdOps2<RL>, ntt_persist_tma_kernel<RL>>("ntt_persist_tma_kernel", 2 * 4096 * sizeof(u64), c, p, st,
+                                                                            vec_out ? 1 : 0);
+        if (sw.v == 6 && vec)
+            return persist_launch<FpFwdOps3<RL>, ntt_persist3_kernel<FpFwdOps3<RL>>>("ntt_persist3_kernel", 2 * FpFwdOps3<RL>::kSmem, c, p, st);
+        if (sw.v == 5 && vec) return ticket_loop<FpFwdOps3<RL>>(c, p, st, true);
+        if (sw.v >= 3) return ticket_loop<FpFwdOps2<RL>>(c, p, st, true);
+        return ticket_loop<FpFwdOps<RL, 0>>(c, p, st, sw.v == 2);
+    }
+    if (!inverse && sw.iv >= 3)
+        return kind == 1 ? ticket_loop<IntFwdOps2<RL, true>>(c, p, st, true) : ticket_loop<IntFwdOps2<RL, false>>(c, p, st, true);
+    if (kind == 1) return inverse ? ticket_loop<IntInvOps<RL, 1>>(c, p, st, sw.v >= 2) : ticket_loop<IntFwdOps<RL, 1>>(c, p, st, sw.v >= 2);
+    return inverse ? ticket_loop<IntInvOps<RL, 2>>(c, p, st, sw.v >= 2) : ticket_loop<IntFwdOps<RL, 2>>(c, p, st, sw.v >= 2);
+}
+
 bool ntt_persist_supported(const Ctx* c) {
-    static const int mode = [] { const char* e = getenv("LGPU_NTT_PERSIST"); return e ? atoi(e) : -1; }();
-    return mode != 0 && c->ring_type == 0 && c->logN >= 13 && c->logN <= 16;
+    return c->ring_type == 0 && c->logN >= 13 && c->logN <= 16;
 }
 
 // kind: 0 = FP64-pipe rows (all rows fp_ok), 1 / 2 = integer rows with / without lazy corrections
 int launch_ntt_persist(const Ctx* c, const RowMap& rm, bool inverse, int kind, CSpan in, Span out, int batch, cudaStream_t st, CSpan mul) {
     if (mul.p && inverse) { set_error("the fused multiply epilogue exists for forward transforms only"); return -1; }
-    const int rl = c->logN - 12;
-    static const int ph1int = [] { const char* e = getenv("LGPU_NTT_PH1INT"); return e ? atoi(e) : 0; }();
-    // LGPU_NTT_PERSIST_V: 1 = first generation (padded tile, CTA barriers, serial ticket), 2 = first-generation tile code under
-    // the claim-ahead loop, 3 (default) = swizzled tile + pair/warp syncs + claim-ahead loop, 4 = 3 + TMA bulk prefetch of the next chunk (no faster
-    // than 3 on the H100: 0.73 vs 0.71 us per limb-transform, profiles/h100_ntt_ab.json), 5 = 3 with the register copy-out (FpFwdOps3), 6 = 5 under
-    // the static-schedule / double-buffered loop
-    static const int pv = [] { const char* e = getenv("LGPU_NTT_PERSIST_V"); return e ? atoi(e) : 3; }();
-    // LGPU_NTT_PERSIST_IV: integer forward tile code, 3 (default) = 512 x 8 swizzled (IntFwdOps2), 2 = 256 x 16 padded (IntFwdOps)
-    static const int piv = [] { const char* e = getenv("LGPU_NTT_PERSIST_IV"); return e ? atoi(e) : 3; }();
-#define PERSIST_CASE(RLV)                                                                                               \
-    case RLV:                                                                                                           \
-        if (kind == 0) {                                                                                                \
-            if (inverse) return pv >= 2 ? persist_launch<FpInvOps<RLV>, true>(c, rm, in, out, batch, st, mul) : persist_launch<FpInvOps<RLV>>(c, rm, in, out, batch, st, mul);                               \
-            if (ph1int) return persist_launch<FpFwdOps<RLV, 1>>(c, rm, in, out, batch, st, mul);                             \
-            if (pv == 4) return persist_launch_tma<RLV>(c, rm, in, out, batch, st, mul);                                     \
-            if (pv == 6 && aligned16(out.p) && even_words(out.row_stride, out.batch_stride) && (!mul.p || (aligned16(mul.p) && even_words(mul.row_stride, mul.batch_stride)))) \
-                return persist_launch3<FpFwdOps3<RLV>>(c, rm, in, out, batch, st, mul);                                      \
-            if (pv == 5 && aligned16(out.p) && even_words(out.row_stride, out.batch_stride) && (!mul.p || (aligned16(mul.p) && even_words(mul.row_stride, mul.batch_stride)))) \
-                return persist_launch<FpFwdOps3<RLV>, true>(c, rm, in, out, batch, st, mul);                                 \
-            if (pv >= 3) return persist_launch<FpFwdOps2<RLV>, true>(c, rm, in, out, batch, st, mul);                        \
-            if (pv == 2) return persist_launch<FpFwdOps<RLV, 0>, true>(c, rm, in, out, batch, st, mul);                      \
-            return persist_launch<FpFwdOps<RLV, 0>>(c, rm, in, out, batch, st, mul);                                         \
-        }                                                                                                               \
-        if (!inverse && piv >= 3) return kind == 1 ? persist_launch<IntFwdOps2<RLV, true>, true>(c, rm, in, out, batch, st, mul)  \
-                                                   : persist_launch<IntFwdOps2<RLV, false>, true>(c, rm, in, out, batch, st, mul); \
-        if (pv >= 2) {                                                                                                  \
-            if (kind == 1) return inverse ? persist_launch<IntInvOps<RLV, 1>, true>(c, rm, in, out, batch, st, mul)          \
-                                          : persist_launch<IntFwdOps<RLV, 1>, true>(c, rm, in, out, batch, st, mul);         \
-            return inverse ? persist_launch<IntInvOps<RLV, 2>, true>(c, rm, in, out, batch, st, mul)                         \
-                           : persist_launch<IntFwdOps<RLV, 2>, true>(c, rm, in, out, batch, st, mul);                        \
-        }                                                                                                               \
-        if (kind == 1) return inverse ? persist_launch<IntInvOps<RLV, 1>>(c, rm, in, out, batch, st, mul)                    \
-                                      : persist_launch<IntFwdOps<RLV, 1>>(c, rm, in, out, batch, st, mul);                   \
-        return inverse ? persist_launch<IntInvOps<RLV, 2>>(c, rm, in, out, batch, st, mul)                                   \
-                       : persist_launch<IntFwdOps<RLV, 2>>(c, rm, in, out, batch, st, mul);
-    switch (rl) {
-        PERSIST_CASE(1) PERSIST_CASE(2) PERSIST_CASE(3) PERSIST_CASE(4)
-        default: break;
+    PersistParams p;
+    p.limbs = c->d_limbs; p.rm = rm; p.in = in.p; p.out = out.p;
+    p.in_rs = in.row_stride; p.in_bs = in.batch_stride; p.out_rs = out.row_stride; p.out_bs = out.batch_stride;
+    p.logN = c->logN; p.batch = batch; p.nLT = rm.nrows * batch;
+    p.mul = mul.p; p.mul_rs = mul.row_stride; p.mul_bs = mul.batch_stride;
+    const bool vec_out = aligned16(out.p) && even_words(out.row_stride, out.batch_stride);
+    const bool vec = vec_out && (!mul.p || (aligned16(mul.p) && even_words(mul.row_stride, mul.batch_stride)));
+    switch (c->logN - 12) {
+        case 1: return persist_dispatch<1>(c, p, inverse, kind, vec, vec_out, st);
+        case 2: return persist_dispatch<2>(c, p, inverse, kind, vec, vec_out, st);
+        case 3: return persist_dispatch<3>(c, p, inverse, kind, vec, vec_out, st);
+        case 4: return persist_dispatch<4>(c, p, inverse, kind, vec, vec_out, st);
     }
-#undef PERSIST_CASE
     set_error("persistent transform: unsupported ring degree");
     return -1;
 }

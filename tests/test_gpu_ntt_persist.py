@@ -136,7 +136,7 @@ def test_edge_primes_match_the_documented_values():
         assert fwd_mask(primes_from(FWD_BOUND + 1, m, 1)[0], logN) != 0
 
 
-# ---- expected kernel launches (ntt.cu: persist_worthwhile, launch_ntt, launch_intt, launch_ntt_mul_montgomery) -------------
+# ---- expected kernel launches (ntt.cu: persistent, transform) ----------------------------------------------------------------
 _FORCED = os.environ.get("LGPU_NTT_PERSIST")
 
 
