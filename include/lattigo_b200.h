@@ -426,6 +426,56 @@ int lgpu_encrypt_zero_sk(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t
  * error samples; sk_in: [nQ][N], sk_out: [nQ + nP][N], NTT + Montgomery. */
 int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t* sk_out, lgpu_gadget_ct* evk, const int64_t* e,
                             void* stream);
+
+/* ---- threshold protocols (multiparty/), Standard ring, NTT domain ------------------------------------------------------------
+ * Sampled polynomials are inputs, as for the encryptor above; every protocol's common reference polynomial comes from the same
+ * samplers keyed by a seed all parties share. PublicKeyGenProtocol.GenShare (multiparty/keygen_cpk.go:70-83) is
+ * lgpu_encrypt_zero_sk at the maximum levels with c1 = crp, is_ntt = is_montgomery = 1. Results keep the reference's
+ * representatives, which need not be canonical (see lgpu_mp_aggregate). Every argument check runs before any launch, also on a
+ * host-only ctx; batch and n_shares are in [1, 65535].
+ *
+ * AggregateShares of any protocol (e.g. keyswitch_sk.go:123-130): out = the left fold agg = shares[0]; agg = Add(agg, shares[k]) in
+ * share order, Add = CRed(a + b) on the wrapping 64-bit sum, exactly as the reference's pairwise calls chain; no final reduction, so
+ * K shares in [0, 2q) give a result in [0, (K + 1) q). shares: HOST array of n_shares device pointers; each share and out are n_polys
+ * blocks of (level_q + 1) Q rows then (level_p + 1) P rows of N words (level_p = -1: Q only). out == shares[0] is allowed, any other
+ * overlap of out and a share is not. One read of every share and one write of out per chunk of 32 pointers. */
+int lgpu_mp_aggregate(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t* const* shares, int n_shares, uint64_t* out, size_t n_polys,
+                      void* stream);
+/* KeySwitchProtocol.GenShare (multiparty/keyswitch_sk.go:85-118), ct.IsNTT: share = MRedLazy(c1, s_in - s_out) + NTT(e), in [0, 2q).
+ * c1: ct.Value[1] of `batch` ciphertexts, level + 1 rows each, batch stride `stride` words; sk_in, sk_out: [nQ (+ nP)][N] NTT +
+ * Montgomery (rows 0..level are read); e: [batch][N] smudging samples (sigma' = sqrt(NoiseFreshSK^2 + sigma_flood^2), bound 6 sigma',
+ * :45-52); share: [batch][level + 1][N]. */
+int lgpu_mp_key_switch_share(lgpu_ctx* ctx, int level, const uint64_t* c1, size_t stride, const uint64_t* sk_in, const uint64_t* sk_out,
+                             const int64_t* e, uint64_t* share, int batch, void* stream);
+/* PublicKeySwitchProtocol.GenShare (multiparty/keyswitch_pk.go:69-105), ct.IsNTT: share = EncryptZero(pk) with (u, e0, e1) as in
+ * lgpu_encrypt_zero_pk (NTT, not Montgomery), then share[0] = CRed(share[0] + MRed(c1, sk)) + NTT(e_flood). c1 as above; sk: [nQ (+ nP)][N];
+ * pk: [2][nQ + nP][N]; u, e0, e1, e_flood: [batch][N]; share: [batch][2][level + 1][N]. */
+int lgpu_mp_public_key_switch_share(lgpu_ctx* ctx, int level, const uint64_t* c1, size_t stride, const uint64_t* sk, const uint64_t* pk,
+                                    const int64_t* u, const int64_t* e0, const int64_t* e1, const int64_t* e_flood, uint64_t* share, int batch,
+                                    void* stream);
+/* Key-generation shares, at the context's maximum levels, for any BaseTwoDecomposition, with or without P. `share` (and `round1`) describe
+ * a gadget layout as for lgpu_gadget_ct (levels, base_two_decomposition, n_digits, n_pw2_max, pw2_sizes); their data is written although
+ * the struct declares it const. A share entry (i, j) is a QP block of nQ + nP rows; a CRP is [n_digits][n_pw2_max][nQ + nP][N] uniform
+ * rows (NTT domain); error samples are [n_digits][n_pw2_max][N]. Entries with j >= pw2_sizes[i] hold unspecified values. Secret keys are
+ * [nQ + nP][N], NTT + Montgomery.
+ *
+ * EvaluationKeyGenProtocol.GenShare (multiparty/keygen_evk.go:86-183): share data [n_digits][n_pw2_max][nQ + nP][N] (one component, like
+ * NewGadgetCiphertext(params, 0, ...)), entry (i, j) = -crp_ij sk_out + e_ij + P 2^(w j) sk_in on the limbs of digit i, NTT + Montgomery.
+ * With gal_els != NULL it is GaloisKeyGenProtocol.GenShare (keygen_gal.go:48-70) for n_keys Galois elements (odd, below 2N) in one call:
+ * key k uses sk_out = AutomorphismNTT(sk_in, gal_els[k]^-1 mod 2N) on Q and P (sk_out is not read), and crp, e and share data carry a
+ * leading key index. gal_els == NULL requires n_keys = 1. */
+int lgpu_mp_evaluation_key_gen_share(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t* sk_out, const uint64_t* gal_els, int n_keys,
+                                     const uint64_t* crp, const int64_t* e, const lgpu_gadget_ct* share, void* stream);
+/* RelinearizationKeyGenProtocol.GenShareRoundOne (multiparty/keygen_relin.go:91-184), plain (not Montgomery) form: share data
+ * [n_digits][n_pw2_max][2][nQ + nP][N], entry (i, j) = (e0_ij + P 2^(w j) s - u crp_ij on the limbs of digit i, NTT(e1_ij) + s crp_ij);
+ * eph_sk_out: the ephemeral secret u (u_small: [N] ternary) as [nQ + nP][N] NTT + Montgomery rows. */
+int lgpu_mp_rkg_share_round_one(lgpu_ctx* ctx, const uint64_t* sk, const int64_t* u_small, const uint64_t* crp, const int64_t* e0,
+                                const int64_t* e1, uint64_t* eph_sk_out, const lgpu_gadget_ct* share, void* stream);
+/* RelinearizationKeyGenProtocol.GenShareRoundTwo (:193-234): round1 is the aggregated round-one share (two components), share data
+ * [n_digits][n_pw2_max][nQ + nP][N] (one component), entry (i, j) = CRed(CRed(MRedLazy(r0_ij, s) + NTT(e2_ij)) + MRed(u - s, r1_ij)), in
+ * [0, 2q). GenRelinearizationKey (:261-276) is MForm of the aggregated round-two share and of round-one component 1. */
+int lgpu_mp_rkg_share_round_two(lgpu_ctx* ctx, const uint64_t* eph_sk, const uint64_t* sk, const lgpu_gadget_ct* round1, const int64_t* e2,
+                                const lgpu_gadget_ct* share, void* stream);
 /* blindrot.Evaluator.BlindRotateCore (core/rgsw/blindrot/evaluator.go:144-229; Algorithm 3 of eprint 2022/198) on one accumulator, in place.
  * a_host: the LWE mask modulo 2N (HOST, n_lwe odd-or-zero words); acc: [2][level+1][N] NTT-domain RLWE accumulator; brk0[j] / brk1[j]:
  * Value[0] / Value[1] of RGSW(X^{s_j}) (HOST arrays of n_lwe key descriptors); gks: the automorphism keys of the window

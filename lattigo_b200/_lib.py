@@ -100,6 +100,12 @@ def lib():
             "lgpu_encrypt_zero_pk": [vp, i, vp, vp, vp, vp, vp, i, i, i, vp],
             "lgpu_encrypt_zero_sk": [vp, i, i, vp, vp, vp, vp, i, i, i, vp],
             "lgpu_gen_evaluation_key": [vp, vp, vp, vp, vp, vp],
+            "lgpu_mp_aggregate": [vp, i, i, vp, i, vp, z, vp],
+            "lgpu_mp_key_switch_share": [vp, i, vp, z, vp, vp, vp, vp, i, vp],
+            "lgpu_mp_public_key_switch_share": [vp, i, vp, z, vp, vp, vp, vp, vp, vp, vp, i, vp],
+            "lgpu_mp_evaluation_key_gen_share": [vp, vp, vp, vp, i, vp, vp, vp, vp],
+            "lgpu_mp_rkg_share_round_one": [vp, vp, vp, vp, vp, vp, vp, vp, vp],
+            "lgpu_mp_rkg_share_round_two": [vp, vp, vp, vp, vp, vp, vp],
             "lgpu_blind_rotate_core": [vp, vp, i, vp, i, vp, vp, vp, i, vp],
             "lgpu_blind_rotation_evaluate": [vp, vp, vp, i, i, vp, i, vp, vp, vp, i, vp, i, i, vp, i, vp],
             "lgpu_ckks_special_fft": [vp, vp, i, i, vp, vp, i, i, z, vp],

@@ -122,4 +122,11 @@ int check_evk(const Ctx* c, int levelQ, const GadgetCt& evk);
 int batch_chunk();
 int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_rescales, u64* out, int batch, cudaStream_t st);
 
+// encrypt.cu, shared with the multiparty shares (multiparty.cu)
+int small_to_rns(const Ctx* c, const RowMap& rm, const long long* in, size_t in_bs, Span out, int batch, cudaStream_t st);
+int encrypt_zero_pk(const Ctx* c, int levelQ, const u64* pk, const long long* u, const long long* e0, const long long* e1, u64* ct_out,
+                    bool is_ntt, bool is_mont, int batch, cudaStream_t st);
+int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, const u64* crp, size_t crp_es, u64* evk, size_t evk_es,
+                       int n_digits, int n_pw2_max, const int* pw2_sizes, const long long* e, bool mont, cudaStream_t st);
+
 }  // namespace lgpu

@@ -169,7 +169,7 @@ static SampleKey make_key(u64 seed, u64 stream) {
     return k;
 }
 
-static int small_to_rns(const Ctx* c, const RowMap& rm, const long long* in, size_t in_bs, Span out, int batch, cudaStream_t st) {
+int small_to_rns(const Ctx* c, const RowMap& rm, const long long* in, size_t in_bs, Span out, int batch, cudaStream_t st) {
     SmallParams p;
     p.limbs = c->d_limbs; p.rm = rm; p.in = in; p.in_bs = in_bs; p.out = out.p; p.rs = out.row_stride; p.bs = out.batch_stride; p.n = c->N;
     count_launch(1);
@@ -255,12 +255,14 @@ int encrypt_zero_pk(const Ctx* c, int levelQ, const u64* pk, const long long* u,
     return 0;
 }
 
-// KeyGenerator.genEvaluationKey (keygenerator.go:287-330) at the maximum levels: on entry component 1 of every evk[i][j] holds the
-// uniform polynomial `a` (QP rows, NTT domain); on return component 0 = -a sk_out + e_ij + P w^j sk_in on the limbs of digit i.
-int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, u64* evk, int n_digits, int n_pw2_max, const int* pw2_sizes,
-                       const long long* e, cudaStream_t st) {
+// KeyGenerator.genEvaluationKey (keygenerator.go:287-330) at the maximum levels, and the share of the multiparty protocols built on it
+// (EvaluationKeyGenProtocol.GenShare, multiparty/keygen_evk.go:86-183; component 0 of RelinearizationKeyGenProtocol.GenShareRoundOne,
+// keygen_relin.go:91-184). Entry (i, j) of evk (stride evk_es words) gets component 0 = -crp_ij sk_out + e_ij + f_j sk_in on the limbs of
+// digit i, crp entry (i, j) at stride crp_es (QP rows, NTT domain). mont: e is taken to Montgomery form and f_j = MForm(P 2^(pw2 j))
+// (key generation, EVKG); otherwise plain e and f_j = P 2^(pw2 j) (RKG round one). Entries with j >= pw2_sizes[i] are unspecified.
+int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, const u64* crp, size_t crp_es, u64* evk, size_t evk_es,
+                       int n_digits, int n_pw2_max, const int* pw2_sizes, const long long* e, bool mont, cudaStream_t st) {
     const int levelQ = c->nQ - 1, levelP = c->nP - 1;
-    const size_t N = c->N, rows = (size_t)c->nQ + c->nP;
     const int nd = levelP >= 0 ? base_rns_decomposition_vector_size(levelQ, levelP) : levelQ + 1;
     if (n_digits != nd) { set_error("evaluation key: n_digits != BaseRNSDecompositionVectorSize(levelQ, levelP)"); return -1; }
     if (n_pw2_max < 1 || n_pw2_max > 64) { set_error("evaluation key: n_pw2_max out of [1, 64]"); return -1; }
@@ -268,11 +270,10 @@ int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_ou
     for (int i = 0; pw2_sizes && i < n_digits; i++)
         if (pw2_sizes[i] < 1 || pw2_sizes[i] > n_pw2_max) { set_error("evaluation key: pw2_sizes[i] out of [1, n_pw2_max]"); return -1; }
     const int entries = n_digits * n_pw2_max;
-    const size_t ebs = 2 * rows * N;
-    if (encrypt_zero_sk(c, levelQ, levelP, sk_out, evk + rows * N, ebs, e, evk, ebs, true, true, entries, st)) return -1;
+    if (encrypt_zero_sk(c, levelQ, levelP, sk_out, const_cast<u64*>(crp), crp_es, e, evk, evk_es, true, mont, entries, st)) return -1;
     GadgetAddParams p;
     memset(&p, 0, sizeof(p));
-    p.limbs = c->d_limbs; p.evk = evk; p.ds = (size_t)n_pw2_max * ebs; p.js = ebs; p.pt = sk_in;
+    p.limbs = c->d_limbs; p.evk = evk; p.ds = (size_t)n_pw2_max * evk_es; p.js = evk_es; p.pt = sk_in;
     p.nq = c->nQ; p.k = levelP >= 0 ? levelP + 1 : 1; p.n = c->N; p.npw2 = n_pw2_max;
     for (int i = 0; i < n_digits; i++) p.npw2_of_digit[i] = (unsigned char)(pw2_sizes ? pw2_sizes[i] : n_pw2_max);
     std::vector<u64> hf((size_t)c->nQ * n_pw2_max);
@@ -281,7 +282,7 @@ int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_ou
         u64 f = 1;
         for (int j = 0; j <= levelP; j++) f = h_mulmod(f, c->P[j] % q, q);
         for (int j = 0; j < n_pw2_max; j++) {
-            hf[(size_t)idx * n_pw2_max + j] = h_mform(f, q);
+            hf[(size_t)idx * n_pw2_max + j] = mont ? h_mform(f, q) : f;
             f = h_mulmod(f, (1ull << pw2) % q, q);
         }
     }
@@ -383,8 +384,10 @@ int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t
     GadgetCt g;
     if (to_gadget_ct(evk, g)) return -1;
     REQUIRE(g.levelQ == ctx->c.nQ - 1 && g.levelP == ctx->c.nP - 1, "evaluation keys are generated at the maximum levels");
-    return gen_evaluation_key(&ctx->c, g.pw2, (const u64*)sk_in, (const u64*)sk_out, (u64*)evk->data, g.ndigits, g.npw2max, g.pw2_sizes,
-                              (const long long*)e, (cudaStream_t)stream);
+    const size_t ebs = (size_t)2 * (ctx->c.nQ + ctx->c.nP) * ctx->c.N;     // component 1 of every entry holds the uniform polynomial
+    u64* data = (u64*)evk->data;
+    return gen_evaluation_key(&ctx->c, g.pw2, (const u64*)sk_in, (const u64*)sk_out, data + ebs / 2, ebs, data, ebs, g.ndigits, g.npw2max, g.pw2_sizes,
+                              (const long long*)e, true, (cudaStream_t)stream);
 }
 
 }  // extern "C"
