@@ -686,6 +686,71 @@ int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int level, int fl
                     size_t pt_stride, size_t values_stride, void* stream);
 
 
+/* ---- multiparty BGV / BFV: collective refresh, encryption-to-shares, shares-to-encryption (multiparty/mpbgv) ----------------------
+ * NTT-domain ciphertexts on the Standard ring, paramsIn == paramsOut, through the encoder handle (t, t^-1 mod q_i, floor(Q/2) and the slot
+ * permutation). An AdditiveShare is n = RingT().N() words per entry ([batch][n], dense); KeySwitch shares, CRPs and aggregates are
+ * [batch][level + 1][N]; sk is [nQ + nP][N] (NTT + Montgomery, rows 0..level used); e is [batch][N] signed. batch <= 65535. Every check
+ * runs before any launch, also on a host-only handle. Results keep the reference's words:
+ *   - E2S and S2E shares lie in [0, 2q) (a KeySwitch share in [0, 2q), then Sub = CRed(a + q - b) or Add = CRed(a + b));
+ *   - RingQ2T at level > 0 with n = N returns ModUpExact's lazy word in [0, 3t); the other branches are canonical. GetShare's
+ *     ring-T Add and the RingT2Q of recrypt take such words as the integers they are, as the reference does.
+ *
+ * lgpu_mpbgv_sample_mask: the mask of EncToShareProtocol.GenShare, ring.UniformSampler over ring T: every word uniform in [0, t), with
+ * the rejection of lgpu_sample_uniform, on the mask domain of the Philox counter (bit 29 of the polynomial word, which no other sampler
+ * sets), so mask streams are disjoint from every other stream of the same seed and id.
+ * lgpu_mpbgv_e2s_share: EncToShareProtocol.GenShare (mpbgv/sharing.go:62-71) at `level` = min(ct level, share level): c1 rows 0..level
+ * at batch stride `stride`; share = Sub(KeySwitch(sk, 0) share, NTT(RingT2Q(level, true, mask))).
+ * lgpu_mpbgv_s2e_share: ShareToEncProtocol.GenShare (:126-143): share = Add(KeySwitch(0, sk) share on the crp, NTT(RingT2Q(mask))).
+ * lgpu_mpbgv_e2s_get_share: EncToShareProtocol.GetShare (:78-91): out = RingQ2T(level, true, INTT(Add(agg, ct0))) [+ secret, ring-T
+ * Add]; secret may be null. ct0 rows 0..level at batch stride `stride`. Refused past the CRT limit of lgpu_bgv_decode.
+ * lgpu_mpbgv_recrypt: the end of MaskedTransformProtocol.Transform (mpbgv/transform.go:173-180): ct_out [batch][2][level + 1][N] gets
+ * c0 = Add(NTT(RingT2Q(level, true, mask)), agg) and c1 = crp.
+ * lgpu_mpbgv_encode_ring_t / lgpu_mpbgv_decode_ring_t: EncodeRingT / DecodeRingT (encoder.go:203-262, :341-374) of n []uint64 values per
+ * entry, the Decode / Encode steps of a MaskedTransformFunc; scale = MetaData.Scale.Uint64(). */
+int lgpu_mpbgv_sample_mask(lgpu_bgv_encoder* enc, uint64_t seed, uint64_t stream_id, uint64_t* mask, int batch, void* stream);
+int lgpu_mpbgv_e2s_share(lgpu_bgv_encoder* enc, int level, const uint64_t* c1, size_t stride, const uint64_t* sk, const int64_t* e,
+                         const uint64_t* mask, uint64_t* share, int batch, void* stream);
+int lgpu_mpbgv_s2e_share(lgpu_bgv_encoder* enc, int level, const uint64_t* crp, const uint64_t* sk, const int64_t* e, const uint64_t* mask,
+                         uint64_t* share, int batch, void* stream);
+int lgpu_mpbgv_e2s_get_share(lgpu_bgv_encoder* enc, int level, const uint64_t* ct0, size_t stride, const uint64_t* agg, const uint64_t* secret,
+                             uint64_t* out, int batch, void* stream);
+int lgpu_mpbgv_recrypt(lgpu_bgv_encoder* enc, int level, const uint64_t* mask, const uint64_t* agg, const uint64_t* crp, uint64_t* ct_out, int batch,
+                       void* stream);
+int lgpu_mpbgv_encode_ring_t(lgpu_bgv_encoder* enc, const uint64_t* values, uint64_t scale, uint64_t* pt, int batch, void* stream);
+int lgpu_mpbgv_decode_ring_t(lgpu_bgv_encoder* enc, const uint64_t* pt, uint64_t scale, uint64_t* values, int batch, void* stream);
+
+
+/* ---- multiparty CKKS: collective refresh, encryption-to-shares, shares-to-encryption (multiparty/mpckks) --------------------------
+ * NTT-domain ciphertexts on the Standard ring, paramsIn == paramsOut, IsMontgomery false. An AdditiveShareBigint is dslots = 2 slots
+ * big integers per entry ([batch][dslots][W], W little-endian two's-complement 64-bit words). W is 4 or 8: the smallest with
+ * 64 W >= bits(q_0) + ... + bits(q_level) + 16 at the E2S level, so sums of up to 2^15 shares stay exact; E2S levels needing more are
+ * refused. Lifted values go to coefficient j N / dslots (SetCoefficientsBigint followed by NTTSparseAndMontgomery, whose output is
+ * the NTT of that spread polynomial). Shares lie in [0, 2q) as for mpbgv. Every check runs before any launch, also on a host-only ctx.
+ *
+ * lgpu_mpckks_sample_mask: bignum.RandInt(prng, 2^log_bound) mapped to [-2^(log_bound-1), 2^(log_bound-1)) (sharing.go GenShare), on
+ * the mask domain of the Philox counter plus bit 28 (disjoint from every other stream, mpbgv masks included); log_bound < 64 W.
+ * lgpu_mpckks_e2s_share: EncToShareProtocol.GenShare at `level` = min(ct level, share level): Sub(KeySwitch(sk, 0) share,
+ * NTT(SetCoefficientsBigint(mask))). Refused with "cannot GenShare: ciphertext level is not large enough for refresh correctness" when
+ * 2^log_bound > Q_level.
+ * lgpu_mpckks_s2e_share: ShareToEncProtocol.GenShare: Add(KeySwitch(0, sk) share on the crp, NTT(SetCoefficientsBigint(secret))). With
+ * scales = {d_lo, d_hi, s_lo, s_hi} (128-bit d = defaultScale, s = inputScaleInt, both > 0) each value is Quo(Mul(v, d), s) first
+ * (RefreshProtocol.GenShare's applyTransformAndScale, truncation toward zero); null: no scaling.
+ * lgpu_mpckks_e2s_get_share: EncToShareProtocol.GetShare: PolyToBigintCentered(INTT(Add(agg, ct0)), gap) [+ secret] into out.
+ * lgpu_mpckks_refresh_finalize: RefreshProtocol.Finalize: GetShare(nil) at level_in, the scaling above, SetCoefficientsBigint at level_out,
+ * NTT, Add(agg_s2e) into c0; c1 = crp. ct_out is [batch][2][level_out + 1][N]. */
+int lgpu_mpckks_sample_mask(lgpu_ctx* ctx, int log_slots, int log_bound, int W, uint64_t seed, uint64_t stream_id, uint64_t* mask, int batch,
+                            void* stream);
+int lgpu_mpckks_e2s_share(lgpu_ctx* ctx, int level, int log_slots, int log_bound, const uint64_t* c1, size_t stride, const uint64_t* sk,
+                          const int64_t* e, const uint64_t* mask, int W, uint64_t* share, int batch, void* stream);
+int lgpu_mpckks_s2e_share(lgpu_ctx* ctx, int level, int log_slots, const uint64_t* crp, const uint64_t* sk, const int64_t* e, const uint64_t* secret,
+                          int W, const uint64_t* scales, uint64_t* share, int batch, void* stream);
+int lgpu_mpckks_e2s_get_share(lgpu_ctx* ctx, int level, int log_slots, const uint64_t* ct0, size_t stride, const uint64_t* agg, const uint64_t* secret,
+                              int W, uint64_t* out, int batch, void* stream);
+int lgpu_mpckks_refresh_finalize(lgpu_ctx* ctx, int level_in, int log_slots, const uint64_t* ct0, size_t stride, const uint64_t* agg_e2s,
+                                 int level_out, const uint64_t* agg_s2e, const uint64_t* crp, int W, const uint64_t* scales, uint64_t* ct_out,
+                                 int batch, void* stream);
+
+
 /* ---- launch accounting / profiling (used by bench.py) ------------------------------------------------------- */
 enum lgpu_kclass {
     LGPU_KCLASS_NTT_FWD = 0,   /* one forward transform of rows x batch polynomials (1 or 2 kernels) */

@@ -15,6 +15,8 @@ from . import wire  # noqa: F401,E402
 from . import rgsw  # noqa: F401,E402
 from . import encryptor  # noqa: F401,E402
 from . import multiparty  # noqa: F401,E402
+from . import mpbgv  # noqa: F401,E402
+from . import mpckks  # noqa: F401,E402
 from . import ckks_fft  # noqa: F401,E402
 from .encoder import Encoder  # noqa: F401,E402
 from .bgv_encoder import BGVEncoder  # noqa: F401,E402

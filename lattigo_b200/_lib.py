@@ -115,6 +115,18 @@ def lib():
             "lgpu_bgv_encoder_destroy": [vp],
             "lgpu_bgv_encode": [vp, vp, i, i, u64, i, vp, i, vp, i, z, z, z, vp],
             "lgpu_bgv_decode": [vp, vp, i, i, u64, vp, i, z, z, vp],
+            "lgpu_mpbgv_sample_mask": [vp, u64, u64, vp, i, vp],
+            "lgpu_mpbgv_e2s_share": [vp, i, vp, z, vp, vp, vp, vp, i, vp],
+            "lgpu_mpbgv_s2e_share": [vp, i, vp, vp, vp, vp, vp, i, vp],
+            "lgpu_mpbgv_e2s_get_share": [vp, i, vp, z, vp, vp, vp, i, vp],
+            "lgpu_mpbgv_recrypt": [vp, i, vp, vp, vp, vp, i, vp],
+            "lgpu_mpbgv_encode_ring_t": [vp, vp, u64, vp, i, vp],
+            "lgpu_mpbgv_decode_ring_t": [vp, vp, u64, vp, i, vp],
+            "lgpu_mpckks_sample_mask": [vp, i, i, i, u64, u64, vp, i, vp],
+            "lgpu_mpckks_e2s_share": [vp, i, i, i, vp, z, vp, vp, vp, i, vp, i, vp],
+            "lgpu_mpckks_s2e_share": [vp, i, i, vp, vp, vp, vp, i, vp, vp, i, vp],
+            "lgpu_mpckks_e2s_get_share": [vp, i, i, vp, z, vp, vp, i, vp, i, vp],
+            "lgpu_mpckks_refresh_finalize": [vp, i, i, vp, z, vp, i, vp, vp, i, vp, vp, i, vp],
             "lgpu_poly_load": [vp, vp, z, vp, i, vp, vp, vp],
             "lgpu_poly_store": [vp, vp, i, vp, z, vp, vp],
             "lgpu_gadget_ct_load": [vp, vp, z, vp, z, vp, vp],

@@ -19,6 +19,7 @@
 #include <vector>
 #include "capi_common.h"
 #include "composite.h"
+#include "bgv_encoder.h"
 #include "crt.cuh"
 #include "modarith.cuh"
 
@@ -58,6 +59,9 @@ __global__ void __launch_bounds__(kBgvThreads) bgv_enc_load_kernel(const u64* __
 // (MRed by MForm(scale mod t): any 64-bit word in, canonical out) and per row: MRed by MForm(t^-1 mod q_i) with tinv (RingT2Q's
 // MulScalarBigint); otherwise BRedAdd mod q_i when a transform or MForm follows (the reference's NTT and MForm of a word below 2^61 are
 // those of its residue, DESIGN.md §3.4), or the literal word; MForm when mont (before the transform: both are linear, the output canonical).
+// RAW (RingT2Q of a ring-T polynomial as it is, the multiparty masks): the ring-T word is lifted as the integer it is, without MulScalar,
+// so a word in [t, 2^64) keeps the reference's lift.
+template <bool RAW = false>
 __global__ void __launch_bounds__(kBgvThreads) bgv_enc_lift_kernel(const u64* __restrict__ src, size_t src_bs, int coeffs, int sgn, int n_values,
                                                                    int log_gap, TMod T, u64 smont, const u64* __restrict__ tinv, int canon,
                                                                    int mont, const LimbConst* __restrict__ limbs, int nrows_q, int limb_p0,
@@ -73,7 +77,8 @@ __global__ void __launch_bounds__(kBgvThreads) bgv_enc_lift_kernel(const u64* __
             w = mred(sgn ? signed_to_t(c, T) : c, smont, T.t, T.qinv);
         }
     } else if ((col & ((1 << log_gap) - 1)) == 0) {
-        w = mred(src[b * src_bs + (col >> log_gap)], smont, T.t, T.qinv);
+        w = src[b * src_bs + (col >> log_gap)];
+        if (!RAW) w = mred(w, smont, T.t, T.qinv);
     }
     for (int r = 0; r < nrows_q + nrows_p; r++) {
         const bool isq = r < nrows_q;
@@ -116,6 +121,9 @@ struct ModUpT {
 // (ring/basis_extension.go:282-308): y_k = MRed(x_k, cinv_k), v = uint64(sum_k float64(y_k) / float64(q_k)) in limb order with IEEE
 // division and no FMA, result = sum_k y_k (Q/q_k) + v (t - Q mod t) mod t. The reference's word is that value plus a multiple of t (its
 // lazy multSum); SubScalarBigint's CRed keeps it congruent and the MulScalar(scale^-1) that follows reduces it, so the residue suffices.
+// RAW (RingQ2T alone, for the multiparty protocols): the reference's own word instead of the residue -- multSum's 128-bit sum of
+// y_k MForm((Q/q_k) mod t), MRedLazy'd, plus v (t - Q mod t) mod t, then SubScalarBigint's CRed: a word in [0, 3t), no MulScalar.
+template <bool RAW = false>
 __global__ void __launch_bounds__(kBgvThreads) bgv_dec_modup_kernel(const u64* __restrict__ src, size_t src_bs, int N, const LimbConst* __restrict__ limbs,
                                                                     const u64* __restrict__ tmul, ModUpT M, TMod T, u64 sinv,
                                                                     u64* __restrict__ out, size_t out_bs) {
@@ -124,16 +132,27 @@ __global__ void __launch_bounds__(kBgvThreads) bgv_dec_modup_kernel(const u64* _
     const size_t b = blockIdx.y;
     const u64* x = src + b * src_bs + j;
     double vf = 0.0;
-    u64 s = 0;
+    u64 s = 0, hi = 0, lo = 0;
     for (int k = 0; k < M.L; k++) {
         const u64 q = limbs[k].q, qinv = limbs[k].qinv;
         u64 a = mred(x[(size_t)k * N], tmul[k], q, qinv);
         a = cred(a + M.half_s[k], q);
         const u64 y = mred(a, M.cinv[k], q, qinv);
         vf = __dadd_rn(vf, __ddiv_rn(__ull2double_rn(y), __ull2double_rn(q)));
-        s = cred(s + mred(y, M.cmod[k], T.t, T.qinv), T.t);
+        if (RAW) {
+            u64 ph, pl;
+            mul128(y, M.cmod[k], ph, pl);
+            lo += pl;
+            hi += ph + (lo < pl);
+        } else {
+            s = cred(s + mred(y, M.cmod[k], T.t, T.qinv), T.t);
+        }
     }
     const u64 v = __double2ull_rz(vf);
+    if (RAW) {
+        out[b * out_bs + j] = cred(mred128_lazy(hi, lo, T.t, T.qinv) + M.vt[v] + T.t - M.half_t, T.t);
+        return;
+    }
     s = cred(s + M.vt[v], T.t);
     s = cred(s + T.t - M.half_t, T.t);
     out[b * out_bs + j] = mred(s, sinv, T.t, T.qinv);
@@ -341,6 +360,78 @@ static void launch_bgv_crt(dim3 grid, cudaStream_t st, const u64* src, size_t sr
     bgv_dec_crt_kernel<W><<<grid, kBgvThreads, 0, st>>>(src, src_bs, N, count, log_gap, C, limbs, tmul, qmod_t, T, sinv, out, out_bs);
 }
 
+namespace lgpu {
+
+int bgv_q2t_check(const lgpu_bgv_encoder* enc, int level, int log_gap) {
+    if (level > 0 && log_gap > 0 && crt_words(enc->ctx->c, level) > kMaxCrtWords) {
+        set_error("the bit lengths of q_0..q_level sum past 4096: the CRT accumulator exceeds 4096 bits");
+        return -1;
+    }
+    return 0;
+}
+
+// RingQ2T(level, scaleDown = true) of coefficient-domain rows into tn-word ring-T entries (coefficients j << log_gap), followed by
+// MulScalar(sinv): the branch choice of encoder.go:429-466 over the three kernels above. setup() stages the CRT table of the big-integer
+// branch once; launch() runs one sub-batch. raw keeps the ModUpExact branch's own word (bgv_dec_modup_kernel<true>, sinv = MForm(1)).
+struct Q2T {
+    const lgpu_bgv_encoder* enc;
+    int level, log_gap, tn, W = 0;
+    bool big;
+    Scratch tab;
+    CrtTab C{};
+    ModUpT M{};
+    u64 qmod_t = 0;
+    Q2T(const lgpu_bgv_encoder* e, int l, int lg, int n) : enc(e), level(l), log_gap(lg), tn(n), big(l > 0 && lg > 0) {}
+    int setup(cudaStream_t st) {
+        const Ctx& c = enc->ctx->c;
+        const TMod& T = enc->tm;
+        if (big) {
+            W = crt_width(crt_words(c, level));
+            std::vector<u64> blob = build_crt(c, level, W);
+            if (tab.alloc(blob.size(), st)) return -1;
+            // pageable source: the call returns once `blob` is staged, so it may die with this function
+            LGPU_CUDA_OK(cudaMemcpyAsync(tab.p, blob.data(), blob.size() * 8, cudaMemcpyHostToDevice, st));
+            const int L = level + 1;
+            C.q = tab.p; C.bhi = tab.p + L; C.blo = tab.p + 2 * L; C.inv = tab.p + 3 * L; C.rq = reinterpret_cast<const double*>(tab.p + 4 * L);
+            C.qhat = tab.p + 5 * L; C.Q = C.qhat + (size_t)L * W; C.Qh = C.Q + W; C.L = L;
+        }
+        qmod_t = 1 % T.t;
+        for (int k = 0; k <= level; k++) qmod_t = h_mulmod(qmod_t, c.Q[k] % T.t, T.t);
+        if (level > 0) {
+            const ModUpSet& s = enc->muc[level];
+            M.cinv = enc->d_blob + s.off_qoverqiinvqi; M.cmod = enc->d_blob + s.off_qoverqimodp; M.vt = enc->d_blob + s.off_vtimesqmodp;
+            M.half_s = enc->d_blob + s.off_half_s; M.half_t = enc->blob[s.off_half_t]; M.L = level + 1;
+        }
+        return 0;
+    }
+    int launch(const u64* src, size_t sstride, u64 sinv, bool raw, u64* out, size_t out_bs, int nb, cudaStream_t st) const {
+        const Ctx& c = enc->ctx->c;
+        const TMod& T = enc->tm;
+        const u64* tmul = enc->d_blob;
+        const int N = c.N;
+        count_launch(1);
+        if (level == 0) {
+            bgv_dec_level0_kernel<<<dim3((tn + kBgvThreads - 1) / kBgvThreads, nb), kBgvThreads, 0, st>>>(
+                src, sstride, tn, log_gap, c.h_limbs[0], enc->blob[0], T, (c.Q[0] >> 1) % T.t, sinv, out, out_bs);
+        } else if (!big) {
+            const dim3 grid((N + kBgvThreads - 1) / kBgvThreads, nb);
+            if (raw) bgv_dec_modup_kernel<true><<<grid, kBgvThreads, 0, st>>>(src, sstride, N, c.d_limbs, tmul, M, T, sinv, out, out_bs);
+            else bgv_dec_modup_kernel<false><<<grid, kBgvThreads, 0, st>>>(src, sstride, N, c.d_limbs, tmul, M, T, sinv, out, out_bs);
+        } else {
+            const dim3 grid((tn + kBgvThreads - 1) / kBgvThreads, nb);
+            switch (W) {
+                case 16: launch_bgv_crt<16>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, out_bs); break;
+                case 32: launch_bgv_crt<32>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, out_bs); break;
+                default: launch_bgv_crt<64>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, out_bs); break;
+            }
+        }
+        LGPU_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+};
+
+}  // namespace lgpu
+
 extern "C" int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int level, int flags, uint64_t scale, uint64_t* values, int batch,
                                size_t pt_stride, size_t values_stride, void* stream) {
     REQUIRE(enc, "null encoder");
@@ -356,34 +447,13 @@ extern "C" int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int le
     REQUIRE(pt && aligned8(pt), "null or misaligned plaintext");
     REQUIRE(values && aligned8(values), "null or misaligned values");
     REQUIRE(batch == 1 || (pt_stride >= (size_t)(level + 1) * N && values_stride >= (size_t)tn), "batch strides smaller than one entry");
-    const bool big = level > 0 && log_gap > 0;
-    const int words = big ? crt_words(c, level) : 0;
-    REQUIRE(words <= kMaxCrtWords, "the bit lengths of q_0..q_level sum past 4096: the CRT accumulator exceeds 4096 bits");
+    if (bgv_q2t_check(enc, level, log_gap)) return -1;
     REQUIRE_DEVICE(ctx);
     const cudaStream_t st = (cudaStream_t)stream;
     const TMod& T = enc->tm;
     const u64 sinv = h_mform(h_powmod(scale % T.t, T.t - 2, T.t), T.t);     // MForm(ModExp(scale, t - 2, t))
-    const u64* tmul = enc->d_blob;
-    Scratch tab;
-    CrtTab C{};
-    const int W = big ? crt_width(words) : 0;
-    if (big) {
-        std::vector<u64> blob = build_crt(c, level, W);
-        if (tab.alloc(blob.size(), st)) return -1;
-        // pageable source: the call returns once `blob` is staged, so it may die with this function
-        LGPU_CUDA_OK(cudaMemcpyAsync(tab.p, blob.data(), blob.size() * 8, cudaMemcpyHostToDevice, st));
-        const int L = level + 1;
-        C.q = tab.p; C.bhi = tab.p + L; C.blo = tab.p + 2 * L; C.inv = tab.p + 3 * L; C.rq = reinterpret_cast<const double*>(tab.p + 4 * L);
-        C.qhat = tab.p + 5 * L; C.Q = C.qhat + (size_t)L * W; C.Qh = C.Q + W; C.L = L;
-    }
-    u64 qmod_t = 1 % T.t;
-    for (int k = 0; k <= level; k++) qmod_t = h_mulmod(qmod_t, c.Q[k] % T.t, T.t);
-    ModUpT M{};
-    if (level > 0) {
-        const ModUpSet& s = enc->muc[level];
-        M.cinv = enc->d_blob + s.off_qoverqiinvqi; M.cmod = enc->d_blob + s.off_qoverqimodp; M.vt = enc->d_blob + s.off_vtimesqmodp;
-        M.half_s = enc->d_blob + s.off_half_s; M.half_t = enc->blob[s.off_half_t]; M.L = level + 1;
-    }
+    Q2T q2t(enc, level, log_gap, tn);
+    if (q2t.setup(st)) return -1;
     const size_t poly = (size_t)(level + 1) * N;
     Scratch tbuf;
     if (tbuf.alloc((size_t)tn * batch, st)) return -1;
@@ -401,23 +471,7 @@ extern "C" int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int le
             if (launch_intt(&c, rm, CSpan{src, (size_t)N, pt_stride}, Span{buf.p, (size_t)N, poly}, nb, NTT_CANONICAL, st)) return -1;
             src = buf.p; sstride = poly;
         }
-        u64* out = tbuf.p + (size_t)k * tn;
-        count_launch(1);
-        if (level == 0) {
-            bgv_dec_level0_kernel<<<dim3((tn + kBgvThreads - 1) / kBgvThreads, nb), kBgvThreads, 0, st>>>(
-                src, sstride, tn, log_gap, c.h_limbs[0], enc->blob[0], T, (c.Q[0] >> 1) % T.t, sinv, out, tn);
-        } else if (!big) {
-            bgv_dec_modup_kernel<<<dim3((N + kBgvThreads - 1) / kBgvThreads, nb), kBgvThreads, 0, st>>>(src, sstride, N, c.d_limbs, tmul, M, T,
-                                                                                                      sinv, out, tn);
-        } else {
-            const dim3 grid((tn + kBgvThreads - 1) / kBgvThreads, nb);
-            switch (W) {
-                case 16: launch_bgv_crt<16>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, tn); break;
-                case 32: launch_bgv_crt<32>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, tn); break;
-                default: launch_bgv_crt<64>(grid, st, src, sstride, N, tn, log_gap, C, c.d_limbs, tmul, qmod_t, T, sinv, out, tn); break;
-            }
-        }
-        LGPU_CUDA_OK(cudaGetLastError());
+        if (q2t.launch(src, sstride, sinv, false, tbuf.p + (size_t)k * tn, tn, nb, st)) return -1;
     }
     if (!coeffs) {
         RowMap rt;
@@ -432,3 +486,54 @@ extern "C" int lgpu_bgv_decode(lgpu_bgv_encoder* enc, const uint64_t* pt, int le
     LGPU_CUDA_OK(cudaGetLastError());
     return 0;
 }
+
+namespace lgpu {
+
+BgvEncInfo bgv_encoder_info(const lgpu_bgv_encoder* e) { return BgvEncInfo{e->ctx, &e->T, e->t, e->n}; }
+
+int bgv_ring_q2t(const lgpu_bgv_encoder* e, int level, const u64* src, size_t src_bs, u64* out, size_t out_bs, int batch, cudaStream_t st) {
+    Q2T q2t(e, level, e->log_gap, e->n);
+    if (q2t.setup(st)) return -1;
+    return q2t.launch(src, src_bs, h_mform(1, e->t), true, out, out_bs, batch, st);
+}
+
+int bgv_ring_t2q(const lgpu_bgv_encoder* e, int level, const u64* pT, size_t pT_bs, u64* out, size_t out_bs, int batch, cudaStream_t st) {
+    const Ctx& c = e->ctx->c;
+    count_launch(1);
+    bgv_enc_lift_kernel<true><<<dim3((c.N + kBgvThreads - 1) / kBgvThreads, batch), kBgvThreads, 0, st>>>(
+        pT, pT_bs, 0, 0, 0, e->log_gap, e->tm, 0, e->d_blob + c.nQ, 0, 0, c.d_limbs, level + 1, c.nQ, 0, out, out_bs, nullptr, 0, c.N);
+    LGPU_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int bgv_encode_ring_t(const lgpu_bgv_encoder* e, const u64* values, size_t vs, u64 scale, u64* pT, int batch, cudaStream_t st) {
+    const int n = e->n;
+    count_launch(1);
+    bgv_enc_load_kernel<<<dim3((n + kBgvThreads - 1) / kBgvThreads, batch), kBgvThreads, 0, st>>>(values, vs, n, 0, n, e->d_perm, e->tm, pT);
+    LGPU_CUDA_OK(cudaGetLastError());
+    RowMap rt;
+    if (make_rowmap(e->T, LGPU_RING_Q, 0, rt)) return -1;
+    const Span P{pT, (size_t)n, (size_t)n};
+    if (launch_intt(&e->T, rt, CSpan{pT, (size_t)n, (size_t)n}, P, batch, NTT_CANONICAL, st)) return -1;
+    return launch_vecop(&e->T, rt, LGPU_OP_MULSCALARMONTGOMERY, CSpan{pT, (size_t)n, (size_t)n}, CSpan{nullptr, 0, 0}, P, batch, nullptr, nullptr,
+                        h_mform(scale % e->t, e->t), 0, n, st);
+}
+
+int bgv_decode_ring_t(const lgpu_bgv_encoder* e, const u64* pT, size_t pT_bs, u64 scale, u64* values, size_t vs, int batch, cudaStream_t st) {
+    const int n = e->n;
+    const u64 t = e->t;
+    Scratch buf;
+    if (buf.alloc((size_t)n * batch, st)) return -1;
+    RowMap rt;
+    if (make_rowmap(e->T, LGPU_RING_Q, 0, rt)) return -1;
+    const Span B{buf.p, (size_t)n, (size_t)n};
+    if (launch_vecop(&e->T, rt, LGPU_OP_MULSCALARMONTGOMERY, CSpan{pT, (size_t)n, pT_bs}, CSpan{nullptr, 0, 0}, B, batch, nullptr, nullptr,
+                     h_mform(h_powmod(scale % t, t - 2, t), t), 0, n, st)) return -1;
+    if (launch_ntt(&e->T, rt, CSpan{buf.p, (size_t)n, (size_t)n}, B, batch, NTT_CANONICAL, st)) return -1;
+    count_launch(1);
+    bgv_dec_store_kernel<<<dim3((n + kBgvThreads - 1) / kBgvThreads, batch), kBgvThreads, 0, st>>>(buf.p, n, e->d_perm, n, 0, t, values, vs);
+    LGPU_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+}  // namespace lgpu

@@ -124,6 +124,10 @@ int mulrelin_tail(const Ctx* c, int level, u64* d, const GadgetCt& rlk, int nb_r
 
 // encrypt.cu, shared with the multiparty shares (multiparty.cu)
 int small_to_rns(const Ctx* c, const RowMap& rm, const long long* in, size_t in_bs, Span out, int batch, cudaStream_t st);
+// batch entries of n words uniform in [0, m) on the mask domain of the Philox counter (the mpbgv masks, mp_refresh.cu)
+int sample_mask(u64 m, int n, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st);
+// batch entries of n values uniform in [-2^(log_bound-1), 2^(log_bound-1)), W two's-complement words each (the mpckks masks)
+int sample_big_mask(int n, int W, int log_bound, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st);
 int encrypt_zero_pk(const Ctx* c, int levelQ, const u64* pk, const long long* u, const long long* e0, const long long* e1, u64* ct_out,
                     bool is_ntt, bool is_mont, int batch, cudaStream_t st);
 int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, const u64* crp, size_t crp_es, u64* evk, size_t evk_es,

@@ -41,6 +41,13 @@ struct SampleKey { unsigned k0, k1, stream; };
 enum SampleKind : unsigned { kKindUniform = 0, kKindTernaryP = 1, kKindTernaryH = 2, kKindGaussian = 3 };
 constexpr unsigned kKindShift = 30;
 static_assert(65535ull * kMaxRows + kMaxRows <= (1ull << kKindShift), "the polynomial index reaches the sampler-kind field");
+// The multiparty masks (sample_mask) are uniform draws whose polynomial word also carries kMaskDomain. Every other draw's polynomial
+// index stays below it, so the mask streams share no Philox input with any other stream, and the four kinds keep their streams.
+constexpr unsigned kMaskDomain = 1u << 29;
+static_assert(65535ull * kMaxRows + kMaxRows <= kMaskDomain, "the polynomial index reaches the mask domain bit");
+// The mpckks masks (sample_big_mask) add kBigMaskDomain, so they share no Philox input with the mpbgv masks either.
+constexpr unsigned kBigMaskDomain = 1u << 28;
+static_assert(65535ull * kMaxRows + kMaxRows <= kBigMaskDomain, "the polynomial index reaches the big-mask domain bit");
 // counter words: (coefficient, polynomial | kind << 30, stream_id mod 2^32, attempt); key: make_key(seed, stream_id)
 __device__ __forceinline__ Ph4 draw(const SampleKey& k, SampleKind kind, unsigned poly, unsigned coeff, unsigned attempt) {
     return philox4x32_10(Ph4{coeff, poly | (unsigned)kind << kKindShift, k.stream, attempt}, k.k0, k.k1);
@@ -69,6 +76,52 @@ __global__ void __launch_bounds__(256) sample_uniform_kernel(UniformParams p) {
         if (v < q) break;
     }
     p.out[(size_t)b * p.bs + (size_t)p.rm.drow[r] * p.rs + i] = v;
+}
+
+// uniform in [0, m) per word, m >= 2: ring.UniformSampler over a one-modulus ring (the masks of mpbgv over ring T), with the uniform
+// kernel's rejection; polynomial word = entry | kMaskDomain
+__global__ void __launch_bounds__(256) sample_mask_kernel(u64* out, size_t bs, int n, u64 m, SampleKey key) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u64 mask = ~0ull >> __clzll((long long)(m - 1));
+    const unsigned poly = blockIdx.y | kMaskDomain;
+    u64 v = 0;
+    for (unsigned a = 0;; a++) {
+        const Ph4 d = draw(key, kKindUniform, poly, (unsigned)i, a);
+        v = (((u64)d.x << 32) | d.y) & mask;
+        if (v < m) break;
+        v = (((u64)d.z << 32) | d.w) & mask;
+        if (v < m) break;
+    }
+    out[(size_t)blockIdx.y * bs + i] = v;
+}
+
+// bignum.RandInt(prng, 2^log_bound) mapped to [-2^(log_bound-1), 2^(log_bound-1)) (value >= 2^(log_bound-1) minus 2^log_bound), as W
+// little-endian two's-complement words per value: attempt a of value i gives words 2a = (x:y) and 2a + 1 = (z:w), bits from log_bound up
+// are the sign extension of bit log_bound - 1. The bound is a power of two, so no draw is rejected. Polynomial word = entry | kMaskDomain
+// | kBigMaskDomain.
+__global__ void __launch_bounds__(256) sample_big_mask_kernel(u64* out, size_t bs, int n, int W, int log_bound, SampleKey key) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned poly = blockIdx.y | kMaskDomain | kBigMaskDomain;
+    u64* o = out + (size_t)blockIdx.y * bs + (size_t)i * W;
+    const int top = (log_bound - 1) >> 6;                      // word holding the sign bit
+    u64 neg = 0;
+    for (int a = 0; 2 * a <= top; a++) {
+        const Ph4 d = draw(key, kKindUniform, poly, (unsigned)i, (unsigned)a);
+        const u64 v[2] = {((u64)d.x << 32) | d.y, ((u64)d.z << 32) | d.w};
+        for (int h = 0; h < 2 && 2 * a + h <= top; h++) {
+            u64 x = v[h];
+            if (2 * a + h == top) {
+                const int b = (log_bound - 1) & 63;            // sign bit position in this word
+                neg = (x >> b) & 1;
+                const u64 low = b == 63 ? ~0ull : ((1ull << (b + 1)) - 1);
+                x = neg ? (x | ~low) : (x & low);
+            }
+            o[2 * a + h] = x;
+        }
+    }
+    for (int w = top + 1; w < W; w++) o[w] = neg ? ~0ull : 0;
 }
 
 // ternary with P(+-1) = prob / 2 each (ring.Ternary{P}, ring/sampler_ternary.go:136-201). u takes 53 bits, so it is exact and
@@ -167,6 +220,20 @@ static SampleKey make_key(u64 seed, u64 stream) {
     SampleKey k;
     k.k0 = (unsigned)seed; k.k1 = (unsigned)(seed >> 32) ^ (unsigned)(stream >> 32) * 0x85EBCA6Bu; k.stream = (unsigned)stream;
     return k;
+}
+
+int sample_mask(u64 m, int n, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st) {
+    count_launch(1);
+    sample_mask_kernel<<<dim3((n + 255) / 256, batch), 256, 0, st>>>(out, bs, n, m, make_key(seed, stream_id));
+    LGPU_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int sample_big_mask(int n, int W, int log_bound, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st) {
+    count_launch(1);
+    sample_big_mask_kernel<<<dim3((n + 255) / 256, batch), 256, 0, st>>>(out, bs, n, W, log_bound, make_key(seed, stream_id));
+    LGPU_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 int small_to_rns(const Ctx* c, const RowMap& rm, const long long* in, size_t in_bs, Span out, int batch, cudaStream_t st) {
