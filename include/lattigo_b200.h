@@ -476,6 +476,15 @@ int lgpu_mp_rkg_share_round_one(lgpu_ctx* ctx, const uint64_t* sk, const int64_t
  * [0, 2q). GenRelinearizationKey (:261-276) is MForm of the aggregated round-two share and of round-one component 1. */
 int lgpu_mp_rkg_share_round_two(lgpu_ctx* ctx, const uint64_t* eph_sk, const uint64_t* sk, const lgpu_gadget_ct* round1, const int64_t* e2,
                                 const lgpu_gadget_ct* share, void* stream);
+/* Thresholdizer.GenShamirSecretShare (multiparty/threshold.go:102-104) for n_points recipients in one pass: share k is
+ * ringqp.Ring.EvalPolyScalar(poly, points[k]) (ring/ringqp/operations.go:92-102) on the Q rows and on the P rows, by Horner's rule
+ * acc = poly[t-1]; acc = CRed(MRed(acc, MForm(points[k])) + poly[i-1]) for i = t-1 .. 1, with the wrapping 64-bit sum and MForm the
+ * Barrett form of the unreduced point, so any 64-bit input word gives the reference's word. poly: [threshold][(level_q + 1) Q rows then
+ * (level_p + 1) P rows][N], coefficient 0 the secret (ShamirPolynomial.Value); points: HOST array of n_points 64-bit points;
+ * shares: [n_points][rows][N], which must not overlap poly. level_p = -1: Q only; threshold and n_points are in [1, 65535]. Reads every
+ * coefficient once per chunk of 8 points: ceil(n_points / 8) threshold + n_points polynomial sizes of traffic. */
+int lgpu_mp_shamir_share(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t* poly, int threshold, const uint64_t* points, int n_points,
+                         uint64_t* shares, void* stream);
 /* blindrot.Evaluator.BlindRotateCore (core/rgsw/blindrot/evaluator.go:144-229; Algorithm 3 of eprint 2022/198) on one accumulator, in place.
  * a_host: the LWE mask modulo 2N (HOST, n_lwe odd-or-zero words); acc: [2][level+1][N] NTT-domain RLWE accumulator; brk0[j] / brk1[j]:
  * Value[0] / Value[1] of RGSW(X^{s_j}) (HOST arrays of n_lwe key descriptors); gks: the automorphism keys of the window

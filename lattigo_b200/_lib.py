@@ -106,6 +106,7 @@ def lib():
             "lgpu_mp_evaluation_key_gen_share": [vp, vp, vp, vp, i, vp, vp, vp, vp],
             "lgpu_mp_rkg_share_round_one": [vp, vp, vp, vp, vp, vp, vp, vp, vp],
             "lgpu_mp_rkg_share_round_two": [vp, vp, vp, vp, vp, vp, vp],
+            "lgpu_mp_shamir_share": [vp, i, i, vp, i, vp, i, vp, vp],
             "lgpu_blind_rotate_core": [vp, vp, i, vp, i, vp, vp, vp, i, vp],
             "lgpu_blind_rotation_evaluate": [vp, vp, vp, i, i, vp, i, vp, vp, vp, i, vp, i, i, vp, i, vp],
             "lgpu_ckks_special_fft": [vp, vp, i, i, vp, vp, i, i, z, vp],

@@ -6,6 +6,7 @@
 //   EvaluationKeyGenProtocol.GenShare                     multiparty/keygen_evk.go:86-183 (gen_evaluation_key, encrypt.cu)
 //   GaloisKeyGenProtocol.GenShare                         multiparty/keygen_gal.go:48-70
 //   RelinearizationKeyGenProtocol.GenShareRoundOne / Two  multiparty/keygen_relin.go:91-234
+//   Thresholdizer.GenShamirSecretShare, many recipients   multiparty/threshold.go:102-104
 // PublicKeyGenProtocol.GenShare is Encryptor.encryptZeroSkFromC1QP with c1 = crp (encrypt.cu), so it has no entry point here.
 // Sampled polynomials are inputs, as in encrypt.cu. Every result keeps the reference's representative, which need not be canonical:
 // a KeySwitch share lies in [0, 2q), and a left fold of K shares by Add = CRed(a + b) grows by up to q per share.
@@ -186,6 +187,85 @@ __global__ void __launch_bounds__(256) mp_rkg_round_two_kernel(RkgTwoParams p) {
     *o = cred(t + mred(d, r0[(size_t)p.rows * p.n + w], L.q, L.qinv), L.q);
 }
 
+// Thresholdizer.GenShamirSecretShare for a list of recipients (multiparty/threshold.go:102-104 -> ringqp.Ring.EvalPolyScalar,
+// ring/ringqp/operations.go:92-102 and ring/operations.go:269-275): share_k = EvalPolyScalar(poly, points[k]) on every Q and P row.
+// Horner's rule from acc = poly[t-1]: acc = CRed(MRed(acc, MForm(x)) + poly[i-1]), the wrapping 64-bit sum of the reference's
+// MulScalar then Add, with MForm the Barrett form of the unreduced point. A thread keeps the accumulators of kShamirPts points in
+// registers and reads each coefficient word once for them, so n points cost ceil(n / kShamirPts) t + n share-sizes of traffic instead
+// of the 2 + 5 (t - 1) per point of the MulScalar / Add chain. blockIdx.z is the chunk of points.
+constexpr int kShamirPts = 8;
+struct ShamirParams {
+    const u64* poly;             // [t][rows][N]
+    u64* shares;                 // [n_points][rows][N]
+    const u64* points;           // [n_points], device
+    const LimbConst* limbs;
+    unsigned char limb[kMaxRows];   // global limb of every row
+    size_t poly_words;           // rows * N: the stride of a coefficient and of a share
+    int t, n_points, n;
+};
+
+template <bool VEC>
+__global__ void __launch_bounds__(256) mp_shamir_share_kernel(const __grid_constant__ ShamirParams p) {
+    constexpr int W = VEC ? 2 : 1;
+    const int i = (blockIdx.x * blockDim.x + threadIdx.x) * W;
+    if (i >= p.n) return;
+    const LimbConst& L = p.limbs[p.limb[blockIdx.y]];
+    const u64 q = L.q, qinv = L.qinv;
+    const int k0 = blockIdx.z * kShamirPts;
+    u64 x[kShamirPts];
+#pragma unroll
+    for (int k = 0; k < kShamirPts; k++)     // a chunk's tail repeats its last point; those results are not stored
+        x[k] = mform(p.points[min(k0 + k, p.n_points - 1)], q, L.bred_hi, L.bred_lo);
+    const size_t off = (size_t)blockIdx.y * p.n + i;
+    const u64* c = p.poly + (size_t)(p.t - 1) * p.poly_words + off;
+    u64 a[W], acc[kShamirPts][W];
+    if (VEC) { const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(c); a[0] = v.x; a[W - 1] = v.y; }
+    else a[0] = *c;
+#pragma unroll
+    for (int k = 0; k < kShamirPts; k++)
+#pragma unroll
+        for (int w = 0; w < W; w++) acc[k][w] = a[w];
+    for (int j = p.t - 1; j > 0; j--) {
+        c -= p.poly_words;
+        if (VEC) { const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(c); a[0] = v.x; a[W - 1] = v.y; }
+        else a[0] = *c;
+#pragma unroll
+        for (int k = 0; k < kShamirPts; k++)
+#pragma unroll
+            for (int w = 0; w < W; w++) acc[k][w] = cred(mred(acc[k][w], x[k], q, qinv) + a[w], q);
+    }
+    u64* o = p.shares + (size_t)k0 * p.poly_words + off;
+#pragma unroll
+    for (int k = 0; k < kShamirPts; k++) {
+        if (k0 + k >= p.n_points) break;
+        if (VEC) *reinterpret_cast<ulonglong2*>(o) = make_ulonglong2(acc[k][0], acc[k][W - 1]);
+        else *o = acc[k][0];
+        o += p.poly_words;
+    }
+}
+
+int mp_shamir_share(const Ctx* c, int levelQ, int levelP, const u64* poly, int t, const u64* points, int n_points, u64* shares, cudaStream_t st) {
+    const int nq = levelQ + 1, np = levelP + 1;
+    ShamirParams p;
+    memset(&p, 0, sizeof(p));
+    for (int r = 0; r < nq; r++) p.limb[r] = (unsigned char)r;
+    for (int r = 0; r < np; r++) p.limb[nq + r] = (unsigned char)(c->nQ + r);
+    Scratch pts;
+    if (pts.alloc((size_t)n_points, st)) return -1;
+    LGPU_CUDA_OK(cudaMemcpyAsync(pts.p, points, (size_t)n_points * sizeof(u64), cudaMemcpyHostToDevice, st));
+    p.poly = poly; p.shares = shares; p.points = pts.p; p.limbs = c->d_limbs;
+    p.poly_words = (size_t)(nq + np) * c->N;
+    p.t = t; p.n_points = n_points; p.n = c->N;
+    const bool vec = AL(poly) && AL(shares);
+    const int W = vec ? 2 : 1;
+    const dim3 grid((c->N / W + 255) / 256, nq + np, (n_points + kShamirPts - 1) / kShamirPts);
+    count_launch(1);
+    if (vec) mp_shamir_share_kernel<true><<<grid, 256, 0, st>>>(p);
+    else mp_shamir_share_kernel<false><<<grid, 256, 0, st>>>(p);
+    LGPU_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 // the gadget layout of a key-generation share at the context's maximum levels
 static int check_share_layout(const Ctx& c, const lgpu_gadget_ct* g, GadgetCt& out) {
     if (to_gadget_ct(g, out, "null share")) return -1;
@@ -220,6 +300,20 @@ int lgpu_mp_aggregate(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t* c
     }
     REQUIRE_DEVICE(ctx);
     return mp_aggregate(&c, level_q, level_p, (const u64* const*)shares, n_shares, (u64*)out, n_polys, (cudaStream_t)stream);
+}
+
+int lgpu_mp_shamir_share(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t* poly, int threshold, const uint64_t* points, int n_points,
+                         uint64_t* shares, void* stream) {
+    REQUIRE(ctx, "null context");
+    const Ctx& c = ctx->c;
+    REQUIRE(level_q >= 0 && level_q < c.nQ && level_p >= -1 && level_p < c.nP, "level out of range");
+    REQUIRE(threshold >= 1 && threshold <= 65535, "threshold out of [1, 65535]");
+    REQUIRE(n_points >= 1 && n_points <= 65535, "n_points out of [1, 65535]");
+    REQUIRE(poly && points && shares, "null argument");
+    const size_t bytes = (size_t)(level_q + 1 + level_p + 1) * c.N * sizeof(u64);
+    REQUIRE(!overlaps(shares, (size_t)n_points * bytes, poly, (size_t)threshold * bytes), "shares overlap the Shamir polynomial");
+    REQUIRE_DEVICE(ctx);
+    return mp_shamir_share(&c, level_q, level_p, (const u64*)poly, threshold, (const u64*)points, n_points, (u64*)shares, (cudaStream_t)stream);
 }
 
 int lgpu_mp_key_switch_share(lgpu_ctx* ctx, int level, const uint64_t* c1, size_t stride, const uint64_t* sk_in, const uint64_t* sk_out,

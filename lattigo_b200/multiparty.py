@@ -2,7 +2,9 @@
 collective public-key generation (PublicKeyGenProtocol, multiparty/keygen_cpk.go), collective relinearization-, evaluation- and
 Galois-key generation (RelinearizationKeyGenProtocol, EvaluationKeyGenProtocol, GaloisKeyGenProtocol: keygen_relin.go, keygen_evk.go,
 keygen_gal.go; at the maximum levels), collective key switching to a secret key (KeySwitchProtocol, keyswitch_sk.go) and to a public key
-(PublicKeySwitchProtocol, keyswitch_pk.go), NTT-domain ciphertexts on the Standard ring.
+(PublicKeySwitchProtocol, keyswitch_pk.go), NTT-domain ciphertexts on the Standard ring; and the t-out-of-N access structure
+(Thresholdizer, Combiner: threshold.go), with which any t of N parties turn their Shamir shares into additive shares of the secret and
+then run the protocols above as t-out-of-t.
 
 Randomness: every protocol instance draws its private samples from one encryptor.Samplers (the party's own seed), and SampleCRP
 draws the common reference polynomial from a Samplers keyed by a seed all parties share, the CRS. These are the device samplers'
@@ -333,3 +335,151 @@ class RelinearizationKeyGenProtocol(_KeyGenBase):
             Ring(self.ctx, RING_P, self.levelP).MForm(p, p)
             flat[:, self.levelQ + 1:] = p
         return self._gadget(data)
+
+
+_MASK64 = (1 << 64) - 1
+
+
+def _mform(a: int, q: int) -> int:
+    """ring.MForm (ring/modular_reduction.go:11-35): a 2^64 mod q in the Barrett form, for any 64-bit a."""
+    r = (1 << 128) // q
+    mhi = (a * (r & _MASK64)) >> 64
+    x = (-(a * (r >> 64) + mhi) * q) & _MASK64
+    return x - q if x >= q else x
+
+
+def _mred_lazy(x: int, y: int, q: int) -> int:
+    """ring.MRedLazy (:88-95): x y 2^-64 in [0, 2q), with the reference's 64-bit wrap."""
+    lo = (x * y) & _MASK64
+    return (((x * y) >> 64) - ((((lo * pow(q, -1, 1 << 64)) & _MASK64) * q) >> 64) + q) & _MASK64
+
+
+def _mred(x: int, y: int, q: int) -> int:
+    r = _mred_lazy(x, y, q)
+    return r - q if r >= q else r
+
+
+def _modexp_montgomery(x: int, e: int, q: int) -> int:
+    """ring.ModexpMontgomery (ring/utils.go:58-69)."""
+    result = _mform(1, q)
+    while e > 0:
+        if e & 1:
+            result = _mred(result, x, q)
+        x = _mred(x, x, q)
+        e >>= 1
+    return result
+
+
+def _point(x) -> int:
+    x = int(x)
+    if not 0 <= x <= _MASK64:
+        raise _lib.LgpuError("a ShamirPublicPoint is a 64-bit unsigned integer")
+    return x
+
+
+class Thresholdizer:
+    """multiparty.Thresholdizer (multiparty/threshold.go:14-113): t-out-of-N Shamir sharing of a ringqp.Poly secret, at the maximum
+    levels. A ShamirPolynomial is a (t, nQ + nP, N) tensor whose block 0 is the secret; a ShamirSecretShare is a (nQ + nP, N) tensor.
+    ShamirPublicPoints are Python ints in [0, 2^64)."""
+
+    def __init__(self, ctx: Context, samplers: Samplers):
+        self.ctx, self.samplers = ctx, samplers
+        self.levelQ, self.levelP = len(ctx.Q) - 1, len(ctx.P) - 1
+        self.rows = len(ctx.Q) + len(ctx.P)
+
+    def GenShamirPolynomial(self, threshold: int, sk, coeffs=None):
+        """A degree threshold - 1 polynomial with constant term sk (NTT + Montgomery, (nQ + nP, N)) and the other coefficients uniform
+        from one UniformQP draw of the party's samplers (coeffs, a (threshold - 1, nQ + nP, N) tensor, replaces the draw), :81-93."""
+        if threshold < 1:
+            raise _lib.LgpuError("threshold should be >= 1")
+        torch = _torch()
+        shape = (self.rows, self.ctx.N)
+        if tuple(sk.shape) != shape:
+            raise _lib.LgpuError("sk is a (nQ + nP, N) tensor")
+        poly = torch.empty((threshold,) + shape, dtype=torch.int64, device=sk.device)
+        poly[0].copy_(sk)
+        if threshold > 1:
+            if coeffs is None:
+                coeffs = self.samplers.UniformQP(self.levelQ, self.levelP, batch=threshold - 1)
+            if tuple(coeffs.shape) != (threshold - 1,) + shape:
+                raise _lib.LgpuError("coeffs is a (threshold - 1, nQ + nP, N) tensor")
+            poly[1:].copy_(coeffs)
+        return poly
+
+    def AllocateThresholdSecretShare(self):
+        return self.ctx.new_poly(self.rows)
+
+    def GenShamirSecretShare(self, recipient, secretPoly):
+        """The share for one recipient, :102-104."""
+        return self.GenShamirSecretShares([recipient], secretPoly)[0]
+
+    def GenShamirSecretShares(self, recipients, secretPoly):
+        """The shares for every recipient in one pass (lgpu_mp_shamir_share): a (len(recipients), nQ + nP, N) tensor."""
+        pts = [_point(r) for r in recipients]
+        if not pts:
+            raise _lib.LgpuError("GenShamirSecretShares needs at least one recipient")
+        if secretPoly.dim() != 3 or tuple(secretPoly.shape[1:]) != (self.rows, self.ctx.N):
+            raise _lib.LgpuError("secretPoly is a (threshold, nQ + nP, N) tensor")
+        shares = _torch().empty((len(pts), self.rows, self.ctx.N), dtype=_torch().int64, device=secretPoly.device)
+        arr = (ctypes.c_uint64 * len(pts))(*pts)
+        _lib.check(_lib.lib().lgpu_mp_shamir_share(self.ctx.h, self.levelQ, self.levelP, _dptr(secretPoly), secretPoly.shape[0], arr, len(pts),
+                                                   _dptr(shares), _stream()))
+        return shares
+
+    def AggregateShares(self, share1, share2=None, *rest):
+        """:106-113, or the whole list of received shares in one call."""
+        return aggregate(self.ctx, self.levelQ, self.levelP, _shares_arg(share1, share2, rest), mismatch="cannot AggregateShares: shares level do not match")
+
+
+class Combiner:
+    """multiparty.Combiner (multiparty/threshold.go:115-179): turns a party's aggregated Shamir share into a t-out-of-t additive share
+    of the secret. The Lagrange scalars are host work on Python ints, word for word the reference's RNS scalars: `one` = MForm(1),
+    lagrangeCoeffs[that] = MulRNSScalar(Inverse(SubRNSScalar(that, this)), that), MulRNSScalar being MRedLazy, so scalars lie in [0, 2q)."""
+
+    def __init__(self, ctx: Context, own, others, threshold: int):
+        self.ctx, self.threshold = ctx, threshold
+        self.moduli = list(ctx.Q) + list(ctx.P)
+        self.one = [_mform(1, q) for q in self.moduli]
+        own = _point(own)
+        self.lagrangeCoeffs = {}
+        for spk in others:
+            spk = _point(spk)
+            if spk != own:
+                self.lagrangeCoeffs[spk] = self._lagrange_coeff(own, spk)
+
+    def _lagrange_coeff(self, this: int, that: int):
+        out = []
+        for q in self.moduli:
+            a, b = that % q, this % q                               # NewRNSScalarFromUInt64
+            d = a + q - b if b > a else a - b                       # SubRNSScalar(that, this)
+            out.append(_mred_lazy(_modexp_montgomery(d, q - 2, q), a, q))   # Inverse, then MulRNSScalar(., that)
+        return out
+
+    def prod(self, activesPoints, ownPoint):
+        """The RNS scalar GenAdditiveShare multiplies the share by: 2^64 prod over the first threshold actives other than ownPoint of
+        that / (that - ownPoint), in [0, 2q)."""
+        if len(activesPoints) < self.threshold:
+            raise _lib.LgpuError("cannot GenAdditiveShare: Not enough active players to combine threshold shares")
+        own = _point(ownPoint)
+        prod = list(self.one)
+        for active in activesPoints[: self.threshold]:
+            active = _point(active)
+            if active != own:
+                c = self.lagrangeCoeffs.get(active)
+                if c is None:
+                    raise _lib.LgpuError("cannot GenAdditiveShare: active point %d is not among the points the Combiner was created with" % active)
+                prod = [_mred_lazy(x, y, q) for x, y, q in zip(prod, c, self.moduli)]
+        return prod
+
+    def GenAdditiveShare(self, activesPoints, ownPoint, ownShare):
+        """MulRNSScalarMontgomery(ownShare, prod) (:148-167) through the existing vector kernel: a (nQ + nP, N) tensor, the party's
+        additive share of the secret, to use as its secret key in the N-out-of-N protocols."""
+        from .ringqp import Poly, RingQP
+        prod = self.prod(activesPoints, ownPoint)
+        nq = len(self.ctx.Q)
+        if tuple(ownShare.shape) != (len(self.moduli), self.ctx.N):
+            raise _lib.LgpuError("ownShare is a (nQ + nP, N) tensor")
+        out = _torch().empty_like(ownShare)
+        P = (lambda t: t[nq:]) if self.ctx.P else (lambda t: None)
+        RingQP(self.ctx).MulRNSScalarMontgomery(Poly(ownShare[:nq], P(ownShare)), prod, Poly(out[:nq], P(out)))
+        return out

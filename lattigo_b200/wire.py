@@ -70,3 +70,25 @@ def store_poly(ctx: Context, poly) -> bytes:
     w = ctypes.c_size_t()
     _lib.check(_lib.lib().lgpu_poly_store(ctx.h, ctypes.c_void_p(poly.data_ptr()), rows, out.ctypes.data, cap, ctypes.byref(w), _stream()))
     return out[: w.value].tobytes()
+
+
+def store_qp_poly(ctx: Context, poly, levelQ: int = None) -> bytes:
+    """ringqp.Poly.MarshalBinary (ring/ringqp/poly.go:90-160) of a (levelQ+1 + levelP+1, N) device tensor, Q rows first: the Q
+    ring.Poly bytes, then the P ring.Poly bytes. Without P rows the P part is the empty ring.Poly, a zero row count."""
+    nq = len(ctx.Q) if levelQ is None else levelQ + 1
+    q = store_poly(ctx, poly[:nq])
+    return q + (store_poly(ctx, poly[nq:]) if poly.shape[0] > nq else bytes(8))
+
+
+def load_qp_poly(ctx: Context, data: bytes):
+    """ringqp.Poly.UnmarshalBinary -> ((Q rows then P rows, N) device tensor, bytes consumed)."""
+    import torch
+    q, used = load_poly(ctx, data, len(ctx.Q))
+    if ctx.P:
+        p, used_p = load_poly(ctx, data[used:], len(ctx.P))
+        return torch.cat([q, p]), used + used_p
+    if len(data) < used + 8:
+        raise _lib.LgpuError("wire: truncated ring.Poly header")
+    if int.from_bytes(data[used: used + 8], "little") != 0:
+        raise _lib.LgpuError("wire: destination polynomial has fewer rows than the encoded one")
+    return q, used + 8
