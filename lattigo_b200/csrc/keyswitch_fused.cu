@@ -924,6 +924,166 @@ __global__ void __launch_bounds__(512, 2) ks_chunk_mac_fp8r_kernel(KsChunkParams
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// K3, FP64 rows, KS_BCT ciphertexts per CTA (the default for batch >= KS_BCT; LGPU_K3_VARIANT = 11 keeps one per CTA).
+// ks_chunk_mac_fp8r_kernel<1> reads both key components of every (digit, row, chunk) once per ciphertext: 64 KB per digit against
+// 32 KB of P1, in 128-bit loads at a 64-byte thread stride (16 L1 wavefronts per warp-wide load), on the L1 / shared-memory path
+// that bounds K3. Here one CTA owns the same (row, chunk) of KS_BCT consecutive ciphertexts: their tiles go through the four
+// radix-8 rounds side by side (one set of twiddle loads and barriers per digit) and each key word, loaded once, feeds the MAC of
+// every ciphertext. Each ciphertext keeps its own accumulators and sums the same terms in the same digit order with the same
+// FP64 operations as ks_chunk_mac_fp8r_kernel<1>, so the results are identical bit for bit.
+// Shared memory: KS_BCT tiles (32 KB each) + KS_BCT x 2 accumulator sets (32 KB each) = 192 KB at KS_BCT = 2, hence one CTA of
+// 512 threads per SM and up to 128 registers per thread; each thread carries the 2 x 8 independent butterfly chains of its two
+// tiles, which keeps as many FP64 operations in flight per SM as two single-ciphertext CTAs did.
+// H100 80GB HBM3 (700 W), headline step: K3 class 17.4 -> 15.8 ms per step, 1 414 -> 1 471 ct/s (profiles/h100_700w_k3_blocked_ab.jsonl).
+// ------------------------------------------------------------------------------------------------------------
+constexpr int KS_BCT = 2;
+__global__ void __launch_bounds__(512, 1) ks_chunk_mac_fp8r_bct_kernel(KsChunkParams p) {
+    constexpr int CL = 12, T = 512, NB = KS_BCT;
+    extern __shared__ u64 smem[];
+    __shared__ __align__(8) u64 s_bar;
+    double* fsm = reinterpret_cast<double*>(smem);                          // tile of ciphertext c at fsm + c * 4096 (XOR-swizzled)
+    // accumulators: ciphertext c, component m, pair j (coefficients 8*tid + 2j, 2j+1) at accd + ((c*2 + m)*4 + j) * T + tid
+    double2* accd = reinterpret_cast<double2*>(smem + NB * 4096);
+    const int b0 = blockIdx.x * NB, chunk = blockIdx.y, tid = threadIdx.x;
+    const int limb = p.rm.limb[blockIdx.z];
+    const int row = p.rm.drow[blockIdx.z];
+    const LimbConst L = p.limbs[limb];
+    const int s1 = p.logN - CL;
+    const int N = 1 << p.logN;
+    const u64 q = L.q, qinv = L.qinv;
+    const double fq = L.fq, fqinv = L.fqinv;
+    const double* tw = L.ftw_fwd;
+    const size_t erow = (size_t)(row < p.nq ? row : p.nQk + (row - p.nq)) * N + ((size_t)chunk << CL);
+    const u64* P1row = p.P1 + (size_t)b0 * p.p1_bs + (size_t)row * N + ((size_t)chunk << CL);
+    const u64* xin = p.cx + (size_t)b0 * p.cx_bs + (size_t)row * p.cx_rs + ((size_t)chunk << CL) + 8 * tid;
+    const int own_d = row < p.nq ? row / p.k : -1;
+    const unsigned bar = smem_addr(&s_bar);
+    if (tid == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(T) : "memory");
+    __syncthreads();
+    u64 tok = 0;
+    bool pending = false;      // a tile read phase is outstanding: wait for it before overwriting the tiles
+    for (int d = 0; d < p.nd; d++) {
+        const bool own = d == own_d;
+        const u64* e0 = p.evk + (size_t)d * p.evk_ds + erow + 8 * tid;
+        const u64* e1 = e0 + p.evk_cs;
+        int dn = d + 1;
+        if (dn == own_d) dn++;
+        double xd[NB][8];
+        // see ks_chunk_mac_fp8r_kernel: keeps the twiddle addresses from being hoisted out of the digit loop
+        const double* twl = tw;
+        int tl = tid;
+        asm volatile("" : "+l"(twl), "+r"(tl));
+        if (!own) {
+            double x[NB][8];
+            {
+#pragma unroll
+                for (int c = 0; c < NB; c++) {
+                    const u64* src = P1row + (size_t)c * p.p1_bs + (size_t)d * p.p1_ds;
+#pragma unroll
+                    for (int k = 0; k < 8; k++) x[c][k] = __longlong_as_double((long long)src[k * T + tid]);
+                }
+                // the next digit's tiles (NB x 32 KB = NB x 256 lines) travel from HBM into L2 while this digit is processed
+                if (KS_L2_PREFETCH && dn < p.nd && tid < 256 * NB)
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(P1row + (size_t)(tid >> 8) * p.p1_bs + (size_t)dn * p.p1_ds + (tid & 255) * 16));
+                double t1[7];
+                fp8_load_tw<0, true>(t1, twl, s1, chunk, tl);       // CTA-uniform: hi = 0
+#pragma unroll
+                for (int c = 0; c < NB; c++) fp8_bflys(x[c], t1, fq, fqinv);
+                if (pending) { mbar_wait(bar, tok); pending = false; }
+#pragma unroll
+                for (int c = 0; c < NB; c++) fp8s_store_r1(fsm + c * 4096, x[c], tid);
+            }
+            double t[7];
+            fp8_load_tw<3, true>(t, twl, s1, chunk, tl);
+            __syncthreads();
+#pragma unroll
+            for (int c = 0; c < NB; c++) fp8s_round2(fsm + c * 4096, t, fq, fqinv, tid);
+            fp8_load_tw<6, true>(t, twl, s1, chunk, tl);
+            fp8s_pair_sync(tid);
+#pragma unroll
+            for (int c = 0; c < NB; c++) fp8s_round3(fsm + c * 4096, t, fq, fqinv, tid);
+            fp8_load_tw<9, true>(t, twl, s1, chunk, tl);
+            __syncwarp();
+#pragma unroll
+            for (int c = 0; c < NB; c++) fp8s_load_r4(fsm + c * 4096, x[c], tid);
+            tok = mbar_arrive(bar);
+            pending = true;
+#pragma unroll
+            for (int c = 0; c < NB; c++) {
+                fp8_bflys(x[c], t, fq, fqinv);
+#pragma unroll
+                for (int k = 0; k < 8; k++) xd[c][k] = x[c][k];
+            }
+        } else {
+#pragma unroll
+            for (int c = 0; c < NB; c++) {
+                u64 xv[8];
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const ulonglong2 v = ldg128(xin + (size_t)c * p.cx_bs + 2 * j);
+                    xv[2 * j] = v.x; xv[2 * j + 1] = v.y;
+                }
+                if ((xv[0] | xv[1] | xv[2] | xv[3] | xv[4] | xv[5] | xv[6] | xv[7]) >> 46) {
+#pragma unroll
+                    for (int k = 0; k < 8; k++) xv[k] = bred_add(xv[k], q, L.bred_hi);
+                }
+#pragma unroll
+                for (int k = 0; k < 8; k++) xd[c][k] = u2d(xv[k]);
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            ulonglong2 k0[2], k1[2];
+#pragma unroll
+            for (int j = 0; j < 2; j++) { k0[j] = ldg128(e0 + 4 * h + 2 * j); k1[j] = ldg128(e1 + 4 * h + 2 * j); }
+            if ((k0[0].x | k0[0].y | k0[1].x | k0[1].y | k1[0].x | k1[0].y | k1[1].x | k1[1].y) >> 46) {
+#pragma unroll
+                for (int j = 0; j < 2; j++) {
+                    k0[j].x = bred_add(k0[j].x, q, L.bred_hi); k0[j].y = bred_add(k0[j].y, q, L.bred_hi);
+                    k1[j].x = bred_add(k1[j].x, q, L.bred_hi); k1[j].y = bred_add(k1[j].y, q, L.bred_hi);
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < 2; j++) {
+                const int pj = 2 * h + j;
+                const double w0x = u2d(k0[j].x), w0y = u2d(k0[j].y), w1x = u2d(k1[j].x), w1y = u2d(k1[j].y);
+#pragma unroll
+                for (int c = 0; c < NB; c++) {
+                    double2 m0, m1;
+                    m0.x = fp_mulmod(xd[c][2 * pj], w0x, fq, fqinv); m0.y = fp_mulmod(xd[c][2 * pj + 1], w0y, fq, fqinv);
+                    m1.x = fp_mulmod(xd[c][2 * pj], w1x, fq, fqinv); m1.y = fp_mulmod(xd[c][2 * pj + 1], w1y, fq, fqinv);
+                    double2* A0 = accd + (size_t)((c * 2 + 0) * 4 + pj) * T + tid;
+                    double2* A1 = accd + (size_t)((c * 2 + 1) * 4 + pj) * T + tid;
+                    if (d != 0) {
+                        const double2 c0 = *A0, c1 = *A1;
+                        m0.x = __dadd_rn(m0.x, c0.x); m0.y = __dadd_rn(m0.y, c0.y);
+                        m1.x = __dadd_rn(m1.x, c1.x); m1.y = __dadd_rn(m1.y, c1.y);
+                    }
+                    *A0 = m0;
+                    *A1 = m1;
+                }
+            }
+        }
+    }
+    const double rinv = u2d(mred(1, 1, q, qinv));      // 2^-64 mod q: takes the Montgomery factor of the key out of the FP64 sums
+#pragma unroll
+    for (int c = 0; c < NB; c++) {
+        u64* o0 = p.acc + (size_t)(b0 + c) * p.acc_bs + (size_t)row * N + ((size_t)chunk << CL) + 8 * tid;
+        u64* o1 = o0 + p.acc_cs;
+#pragma unroll
+        for (int pj = 0; pj < 4; pj++) {
+            const double2 c0 = accd[(size_t)((c * 2 + 0) * 4 + pj) * T + tid];
+            const double2 c1 = accd[(size_t)((c * 2 + 1) * 4 + pj) * T + tid];
+            ulonglong2 r0, r1;
+            r0.x = fp_canon(fp_mulmod(c0.x, rinv, fq, fqinv), fq, fqinv); r0.y = fp_canon(fp_mulmod(c0.y, rinv, fq, fqinv), fq, fqinv);
+            r1.x = fp_canon(fp_mulmod(c1.x, rinv, fq, fqinv), fq, fqinv); r1.y = fp_canon(fp_mulmod(c1.y, rinv, fq, fqinv), fq, fqinv);
+            *reinterpret_cast<ulonglong2*>(o0 + 2 * pj) = r0;
+            *reinterpret_cast<ulonglong2*>(o1 + 2 * pj) = r1;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // K3 for the integer rows (primes above 2^46: q0, the 56 / 60-bit levels of the bootstrapping chains, the 61-bit special primes), same
 // structure as ks_chunk_mac_fp8r_kernel: 512 threads x 8 coefficients, swizzled tile, pair / warp level exchanges, the last radix-8 round
 // and the MAC in registers, split mbarrier between digits. The 256 x 16 kernel it replaces (ks_chunk_mac_kernel<false>, kept as
@@ -1192,13 +1352,29 @@ int gadget_product_multiple_p_fused(const Ctx* c, int levelQ, CSpan cx, CSpan cx
             ProfScope ps(LGPU_KCLASS_FUSED, st, 8.0 * N * batch * nd * (double)fp.nrows, 1);
             if (ks_launch_strided<true>(s1, nsmax, sp, dim3(gx, fp.nrows, nd * batch), st)) return -1;
         }
+        // LGPU_K3_VARIANT: 21 (default) = KS_BCT ciphertexts per CTA (ks_chunk_mac_fp8r_bct_kernel) for the first batch - batch % KS_BCT
+        // ciphertexts and 11 for the rest; 11 = 512 x 8 kernel with the FP64-pipe MAC, one ciphertext per CTA, 10 = integer-pipe MAC, 12 = one
+        // component each, 0 = the 256 x 16 shared-memory-MAC kernel (kept as a cross-check). H100 (700 W), headline step: class 86.9 ms per
+        // 5 steps with 11 against 91.2 with 10 (profiles/h100_switch_ab.md)
+        static const int k3v = [] { const char* e = getenv("LGPU_K3_VARIANT"); return e ? atoi(e) : 21; }();
+        const int nb = k3v == 21 ? batch / KS_BCT : 0, tail = batch - nb * KS_BCT;
         // algorithmic bytes: P1 read once + accumulators written once + evk once per launch
-        ProfScope ps(LGPU_KCLASS_MAC, st, 8.0 * N * fp.nrows * (batch * (double)(nd + 2) + 2.0 * nd), 1);
-        // LGPU_K3_VARIANT: 11 (default) = 512 x 8 kernel with the FP64-pipe MAC, 10 = integer-pipe MAC, 12 = one component each, 0 = the 256 x 16
-        // shared-memory-MAC kernel (kept as a cross-check). H100 (700 W), headline step: class 86.9 ms per 5 steps with 11 against 91.2 with 10
-        // (profiles/h100_switch_ab.md)
-        static const int k3v = [] { const char* e = getenv("LGPU_K3_VARIANT"); return e ? atoi(e) : 11; }();
-        if (k3v == 11) {
+        ProfScope ps(LGPU_KCLASS_MAC, st, 8.0 * N * fp.nrows * (batch * (double)(nd + 2) + 2.0 * nd), k3v == 21 ? (nb > 0) + (tail > 0) : 1);
+        if (k3v == 21) {
+            if (nb) {
+                const size_t smem_b = (size_t)KS_BCT * 3 * 4096 * sizeof(u64);     // KS_BCT tiles + KS_BCT x 2 accumulator sets
+                LGPU_CUDA_OK(cudaFuncSetAttribute(ks_chunk_mac_fp8r_bct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
+                ks_chunk_mac_fp8r_bct_kernel<<<dim3(nb, chunks, fp.nrows), 512, smem_b, st>>>(cp);
+                LGPU_CUDA_OK(cudaGetLastError());
+            }
+            if (tail) {     // the ciphertexts past the last full block, one per CTA
+                KsChunkParams ct = cp;
+                const size_t b0 = (size_t)nb * KS_BCT;
+                ct.P1 += b0 * cp.p1_bs; ct.cx += b0 * cp.cx_bs; ct.acc += b0 * cp.acc_bs;
+                LGPU_CUDA_OK(cudaFuncSetAttribute(ks_chunk_mac_fp8r_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                ks_chunk_mac_fp8r_kernel<1><<<dim3(tail, chunks, fp.nrows), 512, smem, st>>>(ct);
+            }
+        } else if (k3v == 11) {
             LGPU_CUDA_OK(cudaFuncSetAttribute(ks_chunk_mac_fp8r_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             ks_chunk_mac_fp8r_kernel<1><<<dim3(batch, chunks, fp.nrows), 512, smem, st>>>(cp);
         } else if (k3v == 13) {
