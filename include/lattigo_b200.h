@@ -658,6 +658,36 @@ int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const
 int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
                                  const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out, void* stream);
 
+/* ---- polynomial-vector evaluation (Evaluate with a polynomial.PolynomialVector and a Mapping, CKKS and BGV / BFV) ----------------
+ * The program format above plus one op that only these two entry points accept (the scalar entry points refuse it as an unknown op):
+ *   PTLINCOMB outs[i] = sum_k s[i][k] PT[i][k] terms[k] + s[i][n_terms] PT[i][n_terms] on component 0, rows 0..out_levels[i]
+ *            PT[i][k] = plaintext index[i][k] of `pts` (NTT domain, canonical words), or nothing when the index is -1 (the term is
+ *            skipped: odd / even polynomials); s: [n_out][n_terms+1][level+1] per-limb scalars (< q_r), in which the planner folds
+ *            MForm and the reference's scalar multiplications of the baby step (CKKS: the equal-scale q_level products and the ratio
+ *            >= 2 Mul of MulThenAdd; BGV: tMontgomery and matchScalesBinary's r0 / r1); level = max(out_levels); terms are degree 1 at
+ *            or above every output level that uses them; a used plaintext's level is at least its output's level; n_terms <=
+ *            LGPU_POLY_MAX_TERMS, n_out <= LGPU_POLY_MAX_OUTPUTS; the op's `weights` are unused. Outputs are canonical residues, so
+ *            the result equals the reference's Add(res, vector) / MulThenAdd(X^k, vector, res) sequence bit for bit.
+ * A vector program has exactly one PTLINCOMB (every baby step of the call). The kernel holds each power of a batch entry in
+ * registers and stages the plaintext words of a tile of batch entries in shared memory: each power is read once per batch entry and
+ * each plaintext word once per tile; a sub-batch of up to 8 ciphertexts is one tile, larger ones are tiles of 8. Checked before any launch, also on a host-only context or handle: everything the
+ * scalar entry point checks, the plaintext count (1..2^20), every index (-1..n_pt-1) and plaintext level, the stride, every scalar
+ * below its modulus, and no overlap of the plaintext block with ct_in or ct_out. */
+#define LGPU_POLY_PTLINCOMB 5
+typedef struct {
+    const uint64_t* pt;        /* DEVICE, 16-byte aligned: plaintext j at pt + j * pt_stride, rows 0..pt_levels[j] of N words */
+    size_t pt_stride;          /* words, even, >= (max pt_levels + 1) N */
+    int n_pt;
+    const int* pt_levels;      /* HOST [n_pt] */
+    const int* index;          /* HOST [n_out][n_terms + 1]: plaintext of term k of output i (k = n_terms: the constant), or -1 */
+    const uint64_t* scalars;   /* HOST [n_out][n_terms + 1][level + 1] */
+} lgpu_poly_pt_weights;
+int lgpu_ckks_polynomial_vector_evaluate(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                         const lgpu_poly_pt_weights* pts, const lgpu_gadget_ct* rlk, uint64_t* ct_out, void* stream);
+int lgpu_bgv_polynomial_vector_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                        const lgpu_poly_pt_weights* pts, const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out,
+                                        void* stream);
+
 
 /* ---- BGV / BFV encoder (schemes/bgv/encoder.go; BFV uses the same bgv.Encoder) ---------------------------------------
  * lgpu_bgv_encoder_create: the plaintext ring T of bgv.NewParameters (params.go:76-135) and the tables of NewEncoder (encoder.go:49-133)

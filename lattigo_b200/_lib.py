@@ -85,6 +85,8 @@ def lib():
             "lgpu_bgv_destroy": [vp],
             "lgpu_bgv_mulrelin_batch": [vp, i, vp, vp, vp, i, i, vp, i, vp],
             "lgpu_bgv_polynomial_evaluate": [vp, i, vp, i, vp, vp, i, vp, vp],
+            "lgpu_ckks_polynomial_vector_evaluate": [vp, i, vp, i, vp, vp, vp, vp, vp],
+            "lgpu_bgv_polynomial_vector_evaluate": [vp, i, vp, i, vp, vp, vp, i, vp, vp],
             "lgpu_lintrans_evaluate_many": [vp, i, vp, vp, i, vp, vp, vp, i, vp],
             "lgpu_evaluator_automorphism_hoisted_lazy": [vp, i, vp, vp, i, u64, vp, vp, vp, vp, vp, i, z, z, z, vp],
             "lgpu_evaluator_partial_traces_sum": [vp, i, vp, i, i, i, vp, vp, i, vp],

@@ -16,10 +16,14 @@ check passes only when they are equal, and the Add never reaches matchScalesBina
 from __future__ import annotations
 
 import ctypes
+from math import gcd
 from typing import Sequence
 
+import numpy as np
+
 from . import _lib
-from .polyeval import CHEBYSHEV, MONOMIAL, MULRELIN, RESCALE, TENSOR, Program, _Lin, _Planner, _Poly, _Sim, _Sym
+from .polyeval import (CHEBYSHEV, MONOMIAL, MULRELIN, RESCALE, TENSOR, PolynomialVector, PreparedVector, Program, _check_vector, _Lin,
+                       _Planner, _Poly, _pt_block, _Sim, _Sym, _VLin)
 from .ring import _dptr, _stream
 
 U64_MAX = (1 << 64) - 1
@@ -54,6 +58,29 @@ def centred(c: int, t: int) -> int:
     """c mod T (Euclidean), minus T above T/2 (the scalar cases of Add / Mul / MulThenAdd)."""
     c %= t
     return c - t if c > t >> 1 else c
+
+
+def match_scales_binary(scale0: int, scale1: int, t: int):
+    """Evaluator.matchScalesBinary (schemes/bgv/evaluator.go:1569-1615): (r0, r1) with scale0 r0 = scale1 r1 mod t and small centred
+    r0 + r1."""
+    tHalf = t >> 1
+    center = lambda x: t - x if x >= tHalf else x
+    if gcd(scale0, t) != 1:
+        raise ValueError("cannot matchScalesBinary: invalid ciphertext scale: gcd(scale, t) != 1")
+    a, b = t, 0
+    A, B = pow(scale0, t - 2, t) * scale1 % t, 1
+    r0, r1 = A, B
+    e = center(A) + 1
+    while A != 0:
+        q = a // A
+        a, A = A, a % A
+        b, B = B, (t + b - B * q % t) % t
+        if A != 0 and gcd(A, t) == 1:
+            tmp = center(A) + center(B)
+            if tmp < e:
+                e = tmp
+                r0, r1 = A, B
+    return r0, r1
 
 
 class _BGVSim(_Sim):                              # circuits/bgv/polynomial/polynomial_evaluator_sim.go
@@ -94,8 +121,8 @@ class _BGVSim(_Sim):                              # circuits/bgv/polynomial/poly
 
 
 class _BGVPlanner(_Planner):
-    def __init__(self, Q, t, si):
-        super().__init__(Q, 1, 64, None)
+    def __init__(self, Q, t, si, max_slots=0):
+        super().__init__(Q, 1, 64, None, max_slots)
         self.t, self.si = t, si
         self.sim = _BGVSim(self.Q, t, si)
 
@@ -118,13 +145,43 @@ class _BGVPlanner(_Planner):
         self.prog.ops.append(dict(kind=MULRELIN, dst=y.slot, src0=a.slot, src1=b.slot, level=lv))
         return y
 
-    def baby_step(self, pol, pb, level, scale) -> _Lin:
-        if pol.IsEven and not pol.IsOdd and pol.Degree() == 0:
+    @staticmethod
+    def _degree0_check(even, odd, degree):
+        if even and not odd and degree == 0:
             # NewCiphertext(params, 0, level): Mul(b, X^k) then takes the plaintext branch of tensorStandard, which reads X^k's first
             # component only (BGV), and tensorScaleInvariant indexes a second component that is not there (BFV)
             raise ValueError("an even-only polynomial whose giant-step quotient is a constant gives a degree-0 baby step, which the "
                              "reference's Mul does not multiply as a ciphertext; not supported")
+
+    def baby_step(self, pol, pb, level, scale) -> _Lin:
+        self._degree0_check(pol.IsEven, pol.IsOdd, pol.Degree())
         return super().baby_step(pol, pb, level, scale)
+
+    def vec_baby_step(self, pols, pb, level, scale, mapping) -> _VLin:
+        self._degree0_check(all(p.IsEven for p in pols), all(p.IsOdd for p in pols), pols[0].Degree())
+        return super().vec_baby_step(pols, pb, level, scale, mapping)
+
+    # ---- schemes/bgv vector ops: Add(res, []uint64) and MulThenAdd(X^k, []uint64, res) -------------------------------------
+    def vector_coefficient(self, pols, mapping, k):       # CoefficientGetter.GetVectorCoefficient: Coeffs[k].Uint64()
+        out = []
+        for p in pols:
+            if p.Coeffs[k] is None:
+                raise ValueError("nil coefficient %d" % k)
+            out.append(int(p.Coeffs[k]))
+        return out
+
+    def vec_mul_then_add(self, x: _Sym, values, f: _VLin):     # :1148-1180, then mulRelinThenAdd's plaintext branch :1310-1345
+        if x.level < f.level:
+            raise ValueError("baby step above the level of its power X^k is not supported (MulThenAdd would lower res to X^k's level)")
+        t = self.t
+        pt_scale = 1 if x.scale == f.scale else pow(x.scale, t - 2, t) * f.scale % t
+        r0 = 1
+        if x.scale * pt_scale % t != f.scale:       # the scale of op0 (x) pt against opOut's: equal by construction of pt_scale
+            r0, r1 = match_scales_binary(x.scale * pt_scale % t, f.scale, t)
+            f.scale_by([r1 % q for q in f.Q])
+            f.scale = f.scale * r1 % t
+        f.w[x.slot] = (self._pt(values, f.level, pt_scale), [t * r0 % q for q in f.Q])      # MRed(pt, tMontgomery), then r0
+        f.seq.append(("pt", x.slot))
 
     def monomial(self, a: _Sym, b: _Sym, x: _Sym) -> _Sym:      # EvaluateMonomial: Mul(b, X^k) + Add(.., a) as one TENSOR
         if b.deg == 2:
@@ -178,6 +235,37 @@ def plan(Q: Sequence[int], t: int, level: int, scale: int, coeffs: Sequence[int]
     return _BGVPlanner(Q, t, bool(scale_invariant)).evaluate(level, int(scale), p, int(target_scale))
 
 
+def plan_vector(Q: Sequence[int], t: int, level: int, scale: int, pv: PolynomialVector, target_scale: int, scale_invariant: bool = False,
+                max_slots: int = 0) -> Program:
+    """The device program of Evaluate(ct, pv, targetScale) for a PolynomialVector of monomial-basis uint64 polynomials: with a Mapping,
+    every baby step in one PTLINCOMB plus program.plaintexts (slot vectors Encode'd at (level, scale), scale mod t); without one,
+    plan() of Value[0]. max_slots: MaxSlots of the parameters (the length of the slot vectors)."""
+    p0 = pv.Value[0]
+    if pv.Mapping is None and len(pv.Value) == 1:
+        return plan(Q, t, level, scale, p0.coeffs, target_scale, scale_invariant, p0.odd, p0.even, p0.basis)
+    if p0.basis == CHEBYSHEV:
+        raise ValueError("the Chebyshev basis is not supported for BGV polynomial evaluation (uint64 coefficients); use the monomial basis")
+    if p0.basis != MONOMIAL:
+        raise ValueError("basis must be MONOMIAL")
+    t = int(t)
+    for name, s in (("scale", scale), ("target_scale", target_scale)):
+        if not 1 <= int(s) < t:
+            raise ValueError("%s must be an integer in [1, t)" % name)
+    polys = []
+    for q in pv.Value:
+        coeffs = [int(c) for c in q.coeffs]
+        if any(c < 0 or c > U64_MAX for c in coeffs):
+            raise ValueError("coefficients must be uint64")
+        polys.append(_Poly(coeffs, MONOMIAL, q.odd, q.even))
+    if polys[0].Degree() > 255:
+        raise ValueError("degree %d > 255 is not supported" % polys[0].Degree())
+    if pv.Mapping is not None:
+        if max_slots < 1:
+            raise ValueError("max_slots must be the parameters' MaxSlots (>= 1), got %d" % max_slots)
+        _check_vector(pv, max_slots, max_slots)
+    return _BGVPlanner(Q, t, bool(scale_invariant), max_slots).evaluate(level, int(scale), polys[0], int(target_scale), polys[1:], pv.Mapping)
+
+
 class BGVPolynomialEvaluator:
     """polynomial.Evaluator (circuits/bgv/polynomial) over a BGVEvaluator: InvariantTensoring = bgv_evaluator.ScaleInvariant."""
 
@@ -199,6 +287,52 @@ class BGVPolynomialEvaluator:
         out = torch.empty(shape, dtype=torch.int64, device=ct.device)
         self.run(prog, ct, out, b)
         return out, prog.out_level, prog.out_scale
+
+    # ---- PolynomialVector (Evaluate with a Mapping) ----------------------------------------------------------------------
+    def plan_vector(self, level, scale, pv: PolynomialVector, target_scale) -> Program:
+        from .bgv_encoder import plaintext_slots
+        return plan_vector(self.ctx.Q, self.ev.t, level, scale, pv, target_scale, self.InvariantTensoring, plaintext_slots(self.ctx.N, self.ev.t))
+
+    def encode_plaintexts(self, prog: Program, encoder):
+        """The program's slot vectors, Encode'd with lgpu_bgv_encode (EncodeRingT at the plaintext's scale, RingT2Q with t^-1, NTT): one
+        batched call per distinct (level, scale). encoder: a BGVEncoder of the same context and t."""
+        import torch
+        from .bgv_encoder import ENC_NTT, ENC_SCALE_UP, _vp
+        if encoder.t != self.ev.t:
+            raise ValueError("the encoder's plaintext modulus differs from the evaluator's")
+
+        def encode_group(values, level, scale, out_ptr, stride):
+            v = torch.from_numpy(np.ascontiguousarray(values.view(np.int64))).to("cuda:%d" % self.ctx.device)
+            _lib.check(_lib.lib().lgpu_bgv_encode(encoder.h, _vp(v), values.shape[1], ENC_SCALE_UP | ENC_NTT, int(scale), level,
+                                                  ctypes.c_void_p(out_ptr), -1, None, values.shape[0], values.shape[1], stride, 0, _stream()))
+        return _pt_block(self.ctx, prog, encode_group, np.uint64)
+
+    def PrepareVector(self, level, scale, pv: PolynomialVector, target_scale, encoder) -> PreparedVector:
+        """Plans Evaluate(ct, pv, target_scale) for ciphertexts at (level, scale) and encodes its slot vectors on the device."""
+        prog = self.plan_vector(level, scale, pv, target_scale)
+        pt, lv = self.encode_plaintexts(prog, encoder) if pv.Mapping is not None else (None, [])
+        return PreparedVector(prog, pt, lv)
+
+    def RunVector(self, prep: PreparedVector, ct):
+        """Runs a prepared plan on ct (batch, 2, level+1, N) or (2, level+1, N). Returns the output ciphertexts."""
+        import torch
+        b = ct.shape[0] if ct.dim() == 4 else 1
+        shape = (b, 2, prep.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prep.out_level + 1, self.ctx.N)
+        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
+        cp, vw = prep.structs(1)
+        if vw is None:
+            self.run(prep.prog, ct, out, b)
+        else:
+            rlk = self.ev.rlk
+            _lib.check(_lib.lib().lgpu_bgv_polynomial_vector_evaluate(self.ev.h, ct.shape[-2] - 1, _dptr(ct), b, ctypes.byref(cp), ctypes.byref(vw),
+                                                                      rlk.ref() if rlk is not None else None, 1 if self.InvariantTensoring else 0,
+                                                                      _dptr(out), _stream()))
+        return out
+
+    def EvaluateVector(self, ct, scale, pv: PolynomialVector, target_scale, encoder):
+        """Evaluate(ct, PolynomialVector, targetScale) = PrepareVector + RunVector. Returns (ct_out, level, scale)."""
+        prep = self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, encoder)
+        return self.RunVector(prep, ct), prep.out_level, prep.out_scale
 
     def run(self, prog: Program, ct, out, batch: int):
         cp = prog.to_c(1)

@@ -81,6 +81,81 @@ __global__ void __launch_bounds__(256) poly_lincomb_kernel(LincombParams p) {
     }
 }
 
+struct PtLincombParams {
+    const LimbConst* limbs;
+    const u64* w;                        // [limb][n_out][n_terms + 1]: Montgomery factors of the scalars (see validate)
+    const u64* idx;                      // [n_out][n_terms + 1]: plaintext index, or ~0 for a missing weight
+    const u64* pt;                       // plaintext j: pt + j * pt_stride, row r at + r * n
+    size_t pt_stride;
+    int n_out, n_terms, n, nb;
+    const u64* in[kPolyMaxTerms];
+    unsigned in_cs[kPolyMaxTerms], in_bs[kPolyMaxTerms];
+    int in_level[kPolyMaxTerms];
+    u64* out[kPolyMaxOut];
+    unsigned out_cs[kPolyMaxOut], out_bs[kPolyMaxOut];
+    int out_level[kPolyMaxOut];
+};
+
+// out_i[c][j] = sum_k s_ik PT_ik[j] X_k[c][j] (+ s_iK PT_iK[j] on c = 0), rows r <= out_level[i]. A CTA covers 256 / BT coefficients of
+// one row for BT consecutive batch entries (one warp per entry and 32 coefficients); each thread holds the K terms of its entry in
+// registers, as poly_lincomb_kernel does. Per output, the CTA stages m_ik = MRed(PT_ik, S_ik) for its coefficients in shared memory once
+// (S_ik = s_ik 2^128 mod q for a term, so MRed(X, m) = s PT X; S_iK = s_iK 2^64 for the constant), so each plaintext word is read once
+// per BT ciphertexts and each power once per batch entry. Every product is reduced to [0, q) and every add is followed by a conditional
+// subtraction, so outputs are canonical for any K.
+template <int BT>
+__global__ void __launch_bounds__(256) poly_pt_lincomb_kernel(PtLincombParams p) {
+    constexpr int CJ = 256 / BT;
+    extern __shared__ u64 sm[];
+    const int r = blockIdx.y;
+    const int K1 = p.n_terms + 1, wn = p.n_out * K1;
+    u64* ws = sm;                        // [n_out][K1] factors of row r
+    u64* mp = sm + wn;                   // [K1][CJ] the staged m_ik of the current output
+    for (int t = threadIdx.x; t < wn; t += blockDim.x) ws[t] = p.w[(size_t)r * wn + t];
+    const LimbConst L = p.limbs[r];
+    const u64 q = L.q, qinv = L.qinv;
+    const int jl = threadIdx.x % CJ, j0 = blockIdx.x * CJ, j = j0 + jl;
+    const int b = blockIdx.z * BT + threadIdx.x / CJ;
+    const bool act = b < p.nb && j < p.n;
+    const size_t ro = (size_t)r * p.n + j;
+    u64 x0[kPolyMaxTerms], x1[kPolyMaxTerms];
+#pragma unroll
+    for (int k = 0; k < kPolyMaxTerms; k++) {
+        if (k < p.n_terms) {
+            x0[k] = x1[k] = 0;
+            if (act && r <= p.in_level[k]) {
+                const u64* s = p.in[k] + (size_t)b * p.in_bs[k] + ro;
+                x0[k] = s[0];
+                x1[k] = s[p.in_cs[k]];
+            }
+        }
+    }
+    for (int i = 0; i < p.n_out; i++) {
+        if (r > p.out_level[i]) continue;            // uniform over the CTA
+        __syncthreads();                             // ws is loaded; the previous output's mp is consumed
+        for (int t = threadIdx.x; t < K1 * CJ; t += blockDim.x) {
+            const int k = t / CJ, jj = j0 + t % CJ;
+            const u64 id = p.idx[i * K1 + k];
+            u64 v = 0;
+            if (id != ~0ull && jj < p.n) v = mred(p.pt[id * p.pt_stride + (size_t)r * p.n + jj], ws[i * K1 + k], q, qinv);
+            mp[t] = v;
+        }
+        __syncthreads();
+        if (!act) continue;
+        u64 a0 = mp[p.n_terms * CJ + jl], a1 = 0;
+#pragma unroll
+        for (int k = 0; k < kPolyMaxTerms; k++) {
+            if (k < p.n_terms) {
+                const u64 m = mp[k * CJ + jl];
+                a0 = cred(a0 + mred(x0[k], m, q, qinv), q);
+                a1 = cred(a1 + mred(x1[k], m, q, qinv), q);
+            }
+        }
+        u64* o = p.out[i] + (size_t)b * p.out_bs[i] + ro;
+        o[0] = a0;
+        o[p.out_cs[i]] = a1;
+    }
+}
+
 struct PolyTensorParams {
     const LimbConst* limbs;
     const u64* b; size_t b_cs, b_bs;     // degree 1
@@ -167,7 +242,8 @@ struct Plan {           // what validation derives from the program
     std::vector<std::vector<u64>> w;      // per op: device-ready weights (LINCOMB: [limb][out][term+1][2]; TENSOR: [2][level+1] MForm)
 };
 
-int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl) {
+// vw: the plaintext table of the vector entry points; null for the scalar ones, where PTLINCOMB stays an unknown op
+int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, const lgpu_poly_pt_weights* vw = nullptr) {
     REQUIRE(pg && pg->n_ops >= 1 && pg->ops, "empty polynomial program");
     REQUIRE(pg->n_slots >= 2 && pg->n_slots <= (1 << 16), "program slot count out of range");
     REQUIRE(pg->levels_per_rescale >= 1, "levels_per_rescale must be >= 1");
@@ -183,9 +259,60 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl) {
         }
         return true;
     };
+    int n_pt_ops = 0;
     for (int i = 0; i < pg->n_ops; i++) {
         const lgpu_poly_op& o = pg->ops[i];
         REQUIRE(o.level >= 0 && o.level <= level, "program op level out of range");
+        if (o.kind == LGPU_POLY_PTLINCOMB && vw) {
+            REQUIRE(++n_pt_ops == 1, "a vector program has exactly one PTLINCOMB op");
+            REQUIRE(o.n_out >= 1 && o.n_out <= kPolyMaxOut, "PTLINCOMB output count out of range");
+            REQUIRE(o.n_terms >= 0 && o.n_terms <= kPolyMaxTerms, "PTLINCOMB term count out of range (at most LGPU_POLY_MAX_TERMS)");
+            REQUIRE(o.outs && o.out_levels && (o.n_terms == 0 || o.terms), "PTLINCOMB needs outs, out_levels and terms");
+            REQUIRE(vw->n_pt >= 1 && vw->n_pt <= (1 << 20), "plaintext count out of range");
+            REQUIRE(vw->pt && vw->pt_levels && vw->index && vw->scalars, "null plaintext table");
+            REQUIRE_ALIGNED(AL(vw->pt) && vw->pt_stride % 2 == 0);
+            for (int j = 0; j < vw->n_pt; j++) REQUIRE(vw->pt_levels[j] >= 0 && vw->pt_levels[j] < c.nQ, "plaintext level out of range");
+            int mx = -1;
+            for (int k = 0; k < o.n_out; k++) {
+                REQUIRE(o.out_levels[k] >= 0 && o.out_levels[k] <= o.level, "PTLINCOMB output level out of range");
+                mx = std::max(mx, o.out_levels[k]);
+            }
+            REQUIRE(mx == o.level, "PTLINCOMB level must be the maximum of its output levels");
+            int ptmax = 0;
+            for (int j = 0; j < vw->n_pt; j++) ptmax = std::max(ptmax, vw->pt_levels[j]);
+            REQUIRE(vw->pt_stride >= (size_t)(ptmax + 1) * c.N, "plaintext stride below the rows of its plaintexts");
+            for (int t = 0; t < o.n_terms; t++) {
+                REQUIRE(readable(o.terms[t]), "program reads a slot before it is written");
+                REQUIRE(pl.deg[o.terms[t]] == 1, "PTLINCOMB terms must have degree 1");
+                pl.last_use[o.terms[t]] = i;
+            }
+            const int K = o.n_terms + 1, R = o.level + 1;
+            for (int k = 0; k < o.n_out; k++)
+                for (int t = 0; t < K; t++) {
+                    const int id = vw->index[k * K + t];
+                    REQUIRE(id >= -1 && id < vw->n_pt, "plaintext index out of range");
+                    if (id < 0) continue;
+                    REQUIRE(vw->pt_levels[id] >= o.out_levels[k], "PTLINCOMB output uses a plaintext below its level");
+                    REQUIRE(t == o.n_terms || pl.level[o.terms[t]] >= o.out_levels[k], "PTLINCOMB output uses a term below its level");
+                }
+            REQUIRE(w_ok(vw->scalars, (size_t)o.n_out * K * R, R, 1), "PTLINCOMB scalar not below its modulus");
+            for (int k = 0; k < o.n_out; k++) {
+                const int d = o.outs[k];
+                REQUIRE(slot_ok(d) && pl.level[d] < 0 && d != 0, "program writes a slot twice (or slot 0)");
+                pl.deg[d] = 1; pl.level[d] = o.out_levels[k];
+            }
+            // device layout: [limb][out][term] Montgomery factors (s 2^128 for a term, s 2^64 for the constant), then [out][term] indices
+            std::vector<u64>& w = pl.w[i];
+            w.resize((size_t)R * o.n_out * K + (size_t)o.n_out * K);
+            for (int r = 0; r < R; r++)
+                for (int k = 0; k < o.n_out; k++)
+                    for (int t = 0; t < K; t++) {
+                        const u64 v = h_mform(vw->scalars[((size_t)k * K + t) * R + r], c.Q[r]);
+                        w[((size_t)r * o.n_out + k) * K + t] = t < o.n_terms ? h_mform(v, c.Q[r]) : v;
+                    }
+            for (int k = 0; k < o.n_out * K; k++) w[(size_t)R * o.n_out * K + k] = vw->index[k] < 0 ? ~0ull : (u64)vw->index[k];
+            continue;
+        }
         switch (o.kind) {
         case LGPU_POLY_MULRELIN:
         case LGPU_POLY_TENSOR: {
@@ -266,9 +393,10 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl) {
             REQUIRE(false, "unknown polynomial program op");
         }
     }
+    REQUIRE(!vw || n_pt_ops == 1, "a vector program has exactly one PTLINCOMB op");
     REQUIRE(slot_ok(pg->out_slot) && pl.level[pg->out_slot] >= 0 && pl.deg[pg->out_slot] == 1, "program output slot must be a written degree-1 slot");
     const lgpu_poly_op& last = pg->ops[pg->n_ops - 1];
-    const bool last_writes_out = last.kind == LGPU_POLY_LINCOMB ? std::find(last.outs, last.outs + last.n_out, pg->out_slot) != last.outs + last.n_out
+    const bool last_writes_out = last.kind == LGPU_POLY_LINCOMB || last.kind == LGPU_POLY_PTLINCOMB ? std::find(last.outs, last.outs + last.n_out, pg->out_slot) != last.outs + last.n_out
                                                                 : last.dst == pg->out_slot;
     REQUIRE(last_writes_out, "the program's last op must write its output slot");
     return 0;
@@ -286,6 +414,7 @@ struct Runner {
     std::vector<size_t> w_off;
     const BgvState* bgv = nullptr;        // BGV / BFV: the evaluator state; null for CKKS
     bool si = false;                      // BFV: scale-invariant tensoring
+    const lgpu_poly_pt_weights* vw = nullptr;   // the vector entry points' plaintexts
 
     size_t cs(int i) const { return (size_t)(s[i].level + 1) * c->N; }
     size_t bs(int i) const { return (size_t)(s[i].deg + 1) * cs(i); }
@@ -361,6 +490,43 @@ struct Runner {
         return 0;
     }
 
+    // PTLINCOMB: batch tiles of BT = min(8, nb) rounded up to a power of two (1, 2, 4, 8), so a sub-batch of up to 8 ciphertexts is
+    // one tile and reads each plaintext word once; larger sub-batches read it once per 8 ciphertexts
+    int pt_lincomb(int i, u64* out_chunk) {
+        const lgpu_poly_op& o = pg->ops[i];
+        const size_t N = c->N;
+        const int K1 = o.n_terms + 1;
+        PtLincombParams p;
+        p.limbs = c->d_limbs; p.w = d_w + w_off[i]; p.idx = p.w + (size_t)(o.level + 1) * o.n_out * K1;
+        p.pt = (const u64*)vw->pt; p.pt_stride = vw->pt_stride;
+        p.n_out = o.n_out; p.n_terms = o.n_terms; p.n = c->N; p.nb = nb;
+        for (int k = 0; k < o.n_terms; k++) {
+            p.in[k] = s[o.terms[k]].p; p.in_cs[k] = (unsigned)cs(o.terms[k]); p.in_bs[k] = (unsigned)bs(o.terms[k]);
+            p.in_level[k] = s[o.terms[k]].level;
+        }
+        for (int k = 0; k < o.n_out; k++) {
+            const int d = o.outs[k];
+            if (make(d, d == pg->out_slot ? out_chunk : nullptr)) return -1;
+            p.out[k] = s[d].p; p.out_cs[k] = (unsigned)cs(d); p.out_bs[k] = (unsigned)bs(d); p.out_level[k] = o.out_levels[k];
+        }
+        const int bt = nb > 4 ? 8 : nb > 2 ? 4 : nb, cj = 256 / bt, tiles = (nb + bt - 1) / bt;
+        // bytes: powers once per entry, plaintexts once per tile (every (output, term) pair with a plaintext), outputs once
+        double pts = 0;
+        for (int k = 0; k < o.n_out; k++)
+            for (int t = 0; t < K1; t++) pts += vw->index[k * K1 + t] >= 0 ? o.out_levels[k] + 1 : 0;
+        ProfScope ps(LGPU_KCLASS_VECOP, st, 8.0 * N * ((o.level + 1) * 2.0 * nb * o.n_terms + pts * tiles + 2.0 * nb * (o.level + 1) * o.n_out), 1);
+        const dim3 grid((unsigned)((N + cj - 1) / cj), (unsigned)(o.level + 1), (unsigned)tiles);
+        const size_t smem = ((size_t)o.n_out * K1 + (size_t)K1 * cj) * 8;
+        switch (bt) {
+        case 8: poly_pt_lincomb_kernel<8><<<grid, 256, smem, st>>>(p); break;
+        case 4: poly_pt_lincomb_kernel<4><<<grid, 256, smem, st>>>(p); break;
+        case 2: poly_pt_lincomb_kernel<2><<<grid, 256, smem, st>>>(p); break;
+        default: poly_pt_lincomb_kernel<1><<<grid, 256, smem, st>>>(p); break;
+        }
+        LGPU_CUDA_OK(cudaGetLastError());
+        return 0;
+    }
+
     int op(int i, u64* out_chunk) {
         const lgpu_poly_op& o = pg->ops[i];
         const size_t N = c->N;
@@ -402,11 +568,27 @@ struct Runner {
             LGPU_CUDA_OK(cudaGetLastError());
             return 0;
         }
+        case LGPU_POLY_PTLINCOMB:
+            return pt_lincomb(i, out_chunk);
         }
         return 0;
     }
 };
 
+
+// what the BGV / BFV evaluators add to validate(): one modulus per rescale, and for BFV no RESCALE and operands at the op's level
+int bgv_program_checks(const lgpu_poly_program& prog, const Plan& pl, int scale_invariant) {
+    REQUIRE(prog.levels_per_rescale == 1, "levels_per_rescale must be 1 for BGV / BFV (Rescale drops one modulus)");
+    if (!scale_invariant) return 0;
+    for (int i = 0; i < prog.n_ops; i++) {
+        const lgpu_poly_op& o = prog.ops[i];
+        REQUIRE(o.kind != LGPU_POLY_RESCALE, "the scale-invariant (BFV) evaluator does not rescale: RESCALE in a scale_invariant program");
+        // the scale-invariant tensor reads both operands as [batch][2][level+1][N]
+        REQUIRE(!(o.kind == LGPU_POLY_MULRELIN || o.kind == LGPU_POLY_TENSOR) || (pl.level[o.src0] == o.level && pl.level[o.src1] == o.level),
+                "scale-invariant MULRELIN / TENSOR operands must be at the op's level");
+    }
+    return 0;
+}
 
 // the relinearization key, checked at every level a MULRELIN / RELIN uses it
 int program_rlk(const Ctx& c, const lgpu_poly_program* prog, const lgpu_gadget_ct* rlk, GadgetCt& g) {
@@ -421,7 +603,7 @@ int program_rlk(const Ctx& c, const lgpu_poly_program* prog, const lgpu_gadget_c
 
 // runs a validated program over the batch, one batch_chunk() sub-batch at a time
 int run_program(const Ctx& c, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog, const Plan& pl, const GadgetCt& g,
-                const BgvState* bgv, bool si, uint64_t* ct_out, cudaStream_t st) {
+                const BgvState* bgv, bool si, uint64_t* ct_out, cudaStream_t st, const lgpu_poly_pt_weights* vw = nullptr) {
     std::vector<u64> hw;
     std::vector<size_t> off(prog->n_ops, 0);
     for (int i = 0; i < prog->n_ops; i++) { off[i] = hw.size(); hw.insert(hw.end(), pl.w[i].begin(), pl.w[i].end()); }
@@ -435,7 +617,7 @@ int run_program(const Ctx& c, int level, const uint64_t* ct_in, int batch, const
     const int ch = batch_chunk();
     for (int k = 0; k < batch; k += ch) {
         const int nb = std::min(ch, batch - k);
-        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off, bgv, si};
+        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off, bgv, si, vw};
         R.s[0].p = (u64*)ct_in + (size_t)k * ci; R.s[0].deg = 1; R.s[0].level = level;
         u64* out = (u64*)ct_out + (size_t)k * co;
         for (int i = 0; i < prog->n_ops; i++) {
@@ -480,18 +662,64 @@ extern "C" int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint6
     REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
     Plan pl;
     if (validate(c, level, prog, pl)) return -1;
-    REQUIRE(prog->levels_per_rescale == 1, "levels_per_rescale must be 1 for BGV / BFV (Rescale drops one modulus)");
-    if (scale_invariant) {
-        for (int i = 0; i < prog->n_ops; i++) {
-            const lgpu_poly_op& o = prog->ops[i];
-            REQUIRE(o.kind != LGPU_POLY_RESCALE, "the scale-invariant (BFV) evaluator does not rescale: RESCALE in a scale_invariant program");
-            // the scale-invariant tensor reads both operands as [batch][2][level+1][N]
-            REQUIRE(!(o.kind == LGPU_POLY_MULRELIN || o.kind == LGPU_POLY_TENSOR) || (pl.level[o.src0] == o.level && pl.level[o.src1] == o.level),
-                    "scale-invariant MULRELIN / TENSOR operands must be at the op's level");
-        }
-    }
+    if (bgv_program_checks(*prog, pl, scale_invariant)) return -1;
     GadgetCt g{};
     if (program_rlk(c, prog, rlk, g)) return -1;
     REQUIRE_DEVICE(ev->ctx);
     return run_program(c, level, ct_in, batch, prog, pl, g, &ev->s, scale_invariant == 1, ct_out, (cudaStream_t)stream);
+}
+
+namespace lgpu {
+namespace {
+// the plaintext block may not overlap the input or the output ciphertexts
+int check_pt_block(const Ctx& c, int level, const uint64_t* ct_in, int batch, const Plan& pl, const lgpu_poly_program* prog,
+                   const lgpu_poly_pt_weights* vw, const uint64_t* ct_out) {
+    int ptmax = 0;
+    for (int j = 0; j < vw->n_pt; j++) ptmax = std::max(ptmax, vw->pt_levels[j]);
+    const size_t ptb = ((size_t)(vw->n_pt - 1) * vw->pt_stride + (size_t)(ptmax + 1) * c.N) * 8;
+    const size_t inb = (size_t)batch * 2 * (level + 1) * c.N * 8, outb = (size_t)batch * 2 * (pl.level[prog->out_slot] + 1) * c.N * 8;
+    REQUIRE(!overlaps(vw->pt, ptb, ct_in, inb) && !overlaps(vw->pt, ptb, ct_out, outb), "the plaintext block overlaps the input or the output");
+    return 0;
+}
+}  // namespace
+}  // namespace lgpu
+
+extern "C" int lgpu_ckks_polynomial_vector_evaluate(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                                    const lgpu_poly_pt_weights* pts, const lgpu_gadget_ct* rlk, uint64_t* ct_out, void* stream) {
+    REQUIRE(ctx, "null context");
+    const Ctx& c = ctx->c;
+    REQUIRE(c.ring_type == 0, "polynomial evaluation is not supported on the ConjugateInvariant ring");
+    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
+    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
+    REQUIRE(ct_in && ct_out, "null ciphertext");
+    REQUIRE(pts, "null plaintext table");
+    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
+    Plan pl;
+    if (validate(c, level, prog, pl, pts)) return -1;
+    if (check_pt_block(c, level, ct_in, batch, pl, prog, pts, ct_out)) return -1;
+    GadgetCt g{};
+    if (program_rlk(c, prog, rlk, g)) return -1;
+    REQUIRE_DEVICE(ctx);
+    return run_program(c, level, ct_in, batch, prog, pl, g, nullptr, false, ct_out, (cudaStream_t)stream, pts);
+}
+
+extern "C" int lgpu_bgv_polynomial_vector_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
+                                                   const lgpu_poly_pt_weights* pts, const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out,
+                                                   void* stream) {
+    REQUIRE(ev, "null BGV evaluator");
+    REQUIRE(scale_invariant == 0 || scale_invariant == 1, "scale_invariant must be 0 or 1");
+    const Ctx& c = ev->ctx->c;
+    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
+    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
+    REQUIRE(ct_in && ct_out, "null ciphertext");
+    REQUIRE(pts, "null plaintext table");
+    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
+    Plan pl;
+    if (validate(c, level, prog, pl, pts)) return -1;
+    if (bgv_program_checks(*prog, pl, scale_invariant)) return -1;
+    if (check_pt_block(c, level, ct_in, batch, pl, prog, pts, ct_out)) return -1;
+    GadgetCt g{};
+    if (program_rlk(c, prog, rlk, g)) return -1;
+    REQUIRE_DEVICE(ev->ctx);
+    return run_program(c, level, ct_in, batch, prog, pl, g, &ev->s, scale_invariant == 1, ct_out, (cudaStream_t)stream, pts);
 }

@@ -19,6 +19,8 @@ from __future__ import annotations
 
 import ctypes
 from fractions import Fraction
+
+import numpy as np
 from typing import Dict, List, Optional, Sequence
 
 from . import _lib
@@ -26,7 +28,7 @@ from .ring import Context, _dptr, _stream
 
 SCALE_PREC = 128
 MONOMIAL, CHEBYSHEV = 0, 1
-MULRELIN, TENSOR, RELIN, RESCALE, LINCOMB = 0, 1, 2, 3, 4
+MULRELIN, TENSOR, RELIN, RESCALE, LINCOMB, PTLINCOMB = 0, 1, 2, 3, 4, 5
 MAX_TERMS = 16            # LGPU_POLY_MAX_TERMS: powers X^1 .. X^15 for degree <= 255 (OptimalSplit(8) = 4)
 MAX_OUTPUTS = 64          # LGPU_POLY_MAX_OUTPUTS
 
@@ -220,14 +222,42 @@ class _Lin:
         self.const = [[x * m[i] % q for x in row] for i, (row, q) in enumerate(zip(self.const, self.Q))]
 
 
+class _VLin:
+    """A pending plaintext-weighted form (a baby step with a Mapping): w[slot] = (plaintext, s) for the terms and const = (plaintext, s)
+    for component 0, s the per-limb scalar that multiplies the plaintext. seq: the reference's order of the steps the form folds,
+    ("pt", slot or None for the constant) for an added plaintext product and ("mul", m) for a per-limb multiplication of res."""
+
+    def __init__(self, level, scale, Q):
+        self.level, self.scale, self.Q = level, scale, Q[: level + 1]
+        self.w: Dict[int, tuple] = {}
+        self.const = None
+        self.seq: List[tuple] = []
+
+    def scale_by(self, m):
+        self.seq.append(("mul", [int(x) % q for x, q in zip(m, self.Q)]))
+        mul = lambda s: [x * m[i] % q for i, (x, q) in enumerate(zip(s, self.Q))]
+        self.w = {k: (pt, mul(s)) for k, (pt, s) in self.w.items()}
+        if self.const is not None:
+            self.const = (self.const[0], mul(self.const[1]))
+
+
 class Program:
-    """A planned evaluation: ops (dicts), the slot count, the output slot / level / scale."""
+    """A planned evaluation: ops (dicts), the slot count, the output slot / level / scale. A vector program also lists the slot vectors
+    its PTLINCOMB op multiplies: plaintexts[j] = dict(coeffs, level, scale), coeffs[i] the value of the slots of polynomial i, and
+    slot_map[j] the polynomial of slot j (-1: unmapped, 0); values(j) is the vector to encode."""
 
     def __init__(self):
         self.ops: List[dict] = []
         self.n_slots = 1
         self.out_slot = self.out_level = -1
         self.out_scale = Fraction(0)
+        self.plaintexts: List[dict] = []
+        self.slot_map = None
+
+    def values(self, j: int, dtype=np.complex128):
+        """The slot vector of plaintext j (MaxSlots entries)."""
+        table = np.array(list(self.plaintexts[j]["coeffs"]) + [0], dtype=dtype)
+        return table[self.slot_map]
 
     def kinds(self) -> List[int]:
         return [o["kind"] for o in self.ops]
@@ -239,14 +269,17 @@ class Program:
         for i, o in enumerate(self.ops):
             s = ops[i]
             s.kind, s.dst, s.src0, s.src1, s.addend, s.level = o["kind"], o.get("dst", -1), o.get("src0", -1), o.get("src1", -1), o.get("addend", -1), o["level"]
-            if o["kind"] == LINCOMB:
+            if o["kind"] in (LINCOMB, PTLINCOMB):
                 outs = (ctypes.c_int * len(o["outs"]))(*o["outs"])
                 lv = (ctypes.c_int * len(o["outs"]))(*o["out_levels"])
                 terms = (ctypes.c_int * max(1, len(o["terms"])))(*o["terms"])
-                w = (ctypes.c_uint64 * len(o["weights"]))(*o["weights"])
-                keep += [outs, lv, terms, w]
+                keep += [outs, lv, terms]
                 s.n_out, s.n_terms = len(o["outs"]), len(o["terms"])
-                s.outs, s.out_levels, s.terms, s.weights = outs, lv, terms, ctypes.cast(w, ctypes.POINTER(ctypes.c_uint64))
+                s.outs, s.out_levels, s.terms = outs, lv, terms
+                if o["kind"] == LINCOMB:
+                    w = (ctypes.c_uint64 * len(o["weights"]))(*o["weights"])
+                    keep.append(w)
+                    s.weights = ctypes.cast(w, ctypes.POINTER(ctypes.c_uint64))
             elif o["kind"] == TENSOR:
                 w = (ctypes.c_uint64 * len(o["weights"]))(*o["weights"])
                 keep.append(w)
@@ -254,6 +287,23 @@ class Program:
         prog = PolyProgramStruct(self.n_slots, len(self.ops), ops, self.out_slot, levels_per_rescale)
         prog._keep = (ops, keep)
         return prog
+
+
+    def pt_weights_to_c(self, pt_ptr: int, pt_stride: int, pt_levels: Sequence[int]):
+        """The lgpu_poly_pt_weights struct of the program's PTLINCOMB op for plaintexts at device address pt_ptr, pt_stride words apart."""
+        o = [o for o in self.ops if o["kind"] == PTLINCOMB][0]
+        lv = (ctypes.c_int * len(pt_levels))(*pt_levels)
+        idx = (ctypes.c_int * len(o["index"]))(*o["index"])
+        sc = (ctypes.c_uint64 * len(o["scalars"]))(*o["scalars"])
+        st = PolyPtWeightsStruct(ctypes.c_void_p(pt_ptr), pt_stride, len(pt_levels), lv, idx, ctypes.cast(sc, ctypes.POINTER(ctypes.c_uint64)))
+        st._keep = (lv, idx, sc)
+        return st
+
+
+class PolyPtWeightsStruct(ctypes.Structure):
+    """lgpu_poly_pt_weights (include/lattigo_b200.h)."""
+    _fields_ = [("pt", ctypes.c_void_p), ("pt_stride", ctypes.c_size_t), ("n_pt", ctypes.c_int), ("pt_levels", ctypes.POINTER(ctypes.c_int)),
+                ("index", ctypes.POINTER(ctypes.c_int)), ("scalars", ctypes.POINTER(ctypes.c_uint64))]
 
 
 class PolyOpStruct(ctypes.Structure):
@@ -270,8 +320,9 @@ class PolyProgramStruct(ctypes.Structure):
 
 
 class _Planner:
-    def __init__(self, Q, lpr, prec, roots1):
+    def __init__(self, Q, lpr, prec, roots1, max_slots=0):
         self.Q, self.lpr, self.prec, self.roots1 = [int(q) for q in Q], lpr, prec, roots1
+        self.max_slots = max_slots
         self.prog = Program()
 
     def _slot(self):
@@ -453,22 +504,117 @@ class _Planner:
         self.prog.ops.append(dict(kind=TENSOR, dst=y.slot, src0=b.slot, src1=x.slot, addend=a.slot, level=lv, weights=list(rb) + list(ra)))
         return y
 
+    # ---- the baby step of a PolynomialVector with a Mapping (polynomial_evaluator.go:281-320) ------------------------------
+    def _pt(self, values, level, scale) -> int:
+        """A slot vector to encode at (level, scale); returns its plaintext index."""
+        self.prog.plaintexts.append(dict(coeffs=values, level=level, scale=scale))
+        return len(self.prog.plaintexts) - 1
+
+    def set_mapping(self, n_polys, mapping):
+        """slot_map: which polynomial's coefficient each of the MaxSlots slots takes (GetVectorCoefficient writes the polynomials in
+        order, so a later polynomial wins a slot mapped twice); -1 for an unmapped slot."""
+        sm = np.full(self.max_slots, n_polys, dtype=np.int64)
+        for i in range(n_polys):
+            for j in mapping.get(i, ()):
+                sm[j] = i
+        sm[sm == n_polys] = -1
+        self.prog.slot_map = sm
+
+    def vector_coefficient(self, pols, mapping, k):       # CoefficientGetter.GetVectorCoefficient: nil (CKKS) slots encode as 0
+        return [0j if p.Coeffs[k] is None else complex(float(p.Coeffs[k].re), float(p.Coeffs[k].im)) for p in pols]   # Complex128()
+
+    def vec_add(self, f: _VLin, values):                 # Add(res, vector): encoded at res.Scale, added to component 0
+        f.const = (self._pt(values, f.level, f.scale), [1] * (f.level + 1))
+        f.seq.append(("pt", None))
+
+    def _mul_big_float(self, level, v: Fraction):
+        """Mul(ct, *big.Float v) (schemes/ckks/evaluator.go:629-666): the per-limb scalar and the scale it multiplies by."""
+        cm = _to_complex(_C(v, 0, SCALE_PREC), self.prec)
+        if cm.re.denominator == 1:
+            sc = _snew(1)
+        else:
+            sc = _snew(self.Q[level])
+            for i in range(1, self.lpr):
+                sc = _smul(sc, _snew(self.Q[level - i]))
+        re, _ = _rns_scalar(self.Q[: level + 1], sc, cm)
+        return re, sc
+
+    def vec_mul_then_add(self, x: _Sym, values, f: _VLin):     # MulThenAdd(X^k, vector, res): schemes/ckks/evaluator.go:977-1025
+        if x.level < f.level:
+            raise ValueError("baby step above the level of its power X^k is not supported")
+        level = f.level
+        if x.scale == f.scale:
+            sr = _snew(self.Q[level])
+            for i in range(1, self.lpr):
+                sr = _smul(sr, _snew(self.Q[level - i]))
+            f.scale_by(self._int_mul_weight(level, int(sr)))
+            f.scale = _smul(f.scale, sr)
+        elif x.scale < f.scale:
+            sr = _sdiv(f.scale, x.scale)
+        else:
+            raise ValueError("cannot MulThenAdd: op0.Scale > opOut.Scale is not supported")
+        # mulRelinThenAdd (:1081-1170), degree-0 branch: Mul(opOut, ratio) when the ratio to op0.Scale * pt.Scale is >= 2
+        res_scale = _smul(x.scale, sr)
+        if f.scale < res_scale:
+            ratio = _sdiv(res_scale, f.scale)
+            if float(ratio) >= 2.0:
+                m, _ = self._mul_big_float(level, ratio)
+                f.scale_by(m)
+                f.scale = res_scale
+        f.w[x.slot] = (self._pt(values, level, sr), [1] * (level + 1))
+        f.seq.append(("pt", x.slot))
+
+    def vec_baby_step(self, pols, pb, level, scale, mapping) -> _VLin:
+        even, odd = all(p.IsEven for p in pols), all(p.IsOdd for p in pols)      # PolynomialVector.IsEven / IsOdd
+        p0 = pols[0]
+        minDeg = len(p0.Coeffs) - 1 - (1 if even and not odd else 0)
+        f = _VLin(level, scale, self.Q)
+        if even:
+            self.vec_add(f, self.vector_coefficient(pols, mapping, 0))
+        if minDeg == 0:
+            return f
+        for key in range(p0.Degree(), 0, -1):
+            if (not (even or odd)) or (key & 1 == 0 and even) or (key & 1 == 1 and odd):
+                self.vec_mul_then_add(pb[key], self.vector_coefficient(pols, mapping, key), f)
+        return f
+
+    def ptlincomb(self, forms: List[_VLin], outs: List[_Sym]):
+        terms = sorted({k for f in forms for k in f.w})
+        if len(terms) > MAX_TERMS or len(forms) > MAX_OUTPUTS:
+            raise ValueError("polynomial too large for one PTLINCOMB (%d terms, %d outputs)" % (len(terms), len(forms)))
+        L = max(f.level for f in forms)
+        index, scalars = [], []
+        for f in forms:
+            for k in terms + [None]:
+                e = f.const if k is None else f.w.get(k)
+                index.append(-1 if e is None else e[0])
+                for r in range(L + 1):
+                    scalars.append(e[1][r] if e is not None and r <= f.level else 0)
+        # sequence[i]: output i's steps in the reference's order, ("pt", term position, n_terms for the constant) or ("mul", m per
+        # limb); the device runs the folded form, tools that replay the reference's op sequence read this
+        seq = [[("pt", len(terms) if k is None else terms.index(k)) if kind == "pt" else ("mul", k) for kind, k in f.seq] for f in forms]
+        self.prog.ops.append(dict(kind=PTLINCOMB, level=L, outs=[o.slot for o in outs], out_levels=[f.level for f in forms], terms=terms,
+                                  index=index, scalars=scalars, sequence=seq))
+
     def _sim(self) -> _Sim:
         return _Sim(self.Q, self.lpr)
 
-    def evaluate(self, level, scale, p: _Poly, target_scale) -> Program:
+    def evaluate(self, level, scale, p: _Poly, target_scale, others=(), mapping=None) -> Program:
         """The scheme-independent part of Evaluate (common/polynomial/polynomial_evaluator.go:29-161): level check, power basis,
-        Paterson-Stockmeyer split on the scheme's simEvaluator, every baby step in one LINCOMB, the giant steps, the final
-        Relinearize / Rescale. Scale values are the scheme's (Fractions for CKKS, ints mod t for BGV)."""
+        Paterson-Stockmeyer split on the scheme's simEvaluator, every baby step in one LINCOMB (one PTLINCOMB with a Mapping), the
+        giant steps, the final Relinearize / Rescale. Scale values are the scheme's (Fractions for CKKS, ints mod t for BGV).
+        others: the PolynomialVector's polynomials after p = Value[0]; the power basis takes their odd / even flags OR-ed, the baby
+        steps AND-ed, and each is split on its own."""
         if p.Degree() < 1:
             raise ValueError("the polynomial must have degree >= 1")
+        pols = [p] + list(others)
         pb: Dict[int, _Sym] = {1: _Sym(0, level, scale, 1)}
         depth = (p.Degree() - 1).bit_length()
         if level < self.lpr * depth:
             raise ValueError("%d levels < %d log(d) -> cannot evaluate poly" % (level, self.lpr * depth))
         logDegree = p.Degree().bit_length()
         logSplit = optimal_split(logDegree)
-        odd, even = p.IsOdd, p.IsEven
+        odd, even = any(q.IsOdd for q in pols), any(q.IsEven for q in pols)
         self.gen_power(pb, p.Basis, 1 << (logDegree - 1))
         for i in range((1 << logSplit) - 1, 2, -1):
             if (not (even or odd)) or (i & 1 == 0 and even) or (i & 1 == 1 and odd):
@@ -479,11 +625,19 @@ class _Planner:
         sim.gen_power(spb, 1 << logDegree)
         for i in range((1 << logSplit) - 1, 2, -1):
             sim.gen_power(spb, i)
-        ps, _ = sim.recurse(logSplit, level - sim.depth(p.Degree()), p, spb, target_scale)
-        # every baby step in one LINCOMB
-        forms = [self.baby_step(bs, pb, bs.Level, bs.Scale) for bs in ps]
-        outs = [_Sym(self._slot(), f.level, f.scale, 1) for f in forms]
-        self.lincomb(forms, outs)
+        pss = [sim.recurse(logSplit, level - sim.depth(p.Degree()), q, spb, target_scale)[0] for q in pols]
+        ps = pss[0]
+        if mapping is not None:                                    # every baby step in one PTLINCOMB
+            self.set_mapping(len(pols), mapping)
+            forms = [self.vec_baby_step([s[i] for s in pss], pb, bs.Level, bs.Scale, mapping) for i, bs in enumerate(ps)]
+            outs = [_Sym(self._slot(), f.level, f.scale, 1) for f in forms]
+            self.ptlincomb(forms, outs)
+        else:                                                      # every baby step in one LINCOMB
+            for i, bs in enumerate(ps):                            # GetSingleCoefficient of Value[0] under the vector's AND-ed flags
+                bs.IsEven, bs.IsOdd = all(s[i].IsEven for s in pss), all(s[i].IsOdd for s in pss)
+            forms = [self.baby_step(bs, pb, bs.Level, bs.Scale) for bs in ps]
+            outs = [_Sym(self._slot(), f.level, f.scale, 1) for f in forms]
+            self.lincomb(forms, outs)
         split = len(ps)
         babySteps = [None] * split
         for i in range(split):
@@ -542,6 +696,119 @@ def plan(Q: Sequence[int], level: int, scale, coeffs, basis: int, target_scale, 
     return _Planner(Q, levels_per_rescale, encoding_precision, roots1).evaluate(level, Fraction(scale), p, Fraction(target_scale))
 
 
+class Polynomial:
+    """bignum.NewPolynomial(basis, coeffs, nil) with its IsOdd / IsEven flags (polynomial.NewPolynomial)."""
+
+    def __init__(self, coeffs, basis: int = MONOMIAL, odd: bool = True, even: bool = True):
+        self.coeffs, self.basis, self.odd, self.even = list(coeffs), basis, odd, even
+
+    def Degree(self):
+        return len(self.coeffs) - 1
+
+
+class PolynomialVector:
+    """polynomial.PolynomialVector: Value (the polynomials) and Mapping {i: slots that take polynomial i} or None."""
+
+    def __init__(self, value: Sequence[Polynomial], mapping: Optional[Dict[int, Sequence[int]]]):
+        self.Value, self.Mapping = list(value), mapping
+
+
+def NewPolynomialVector(polys: Sequence[Polynomial], mapping) -> PolynomialVector:
+    """polynomial.NewPolynomialVector (circuits/common/polynomial/polynomial.go:165-195), with the reference's errors."""
+    if not polys:
+        raise ValueError("a polynomial vector needs at least one polynomial")
+    maxDeg = max(p.Degree() for p in polys)
+    basis = polys[-1].basis
+    for p in polys:
+        if basis != p.basis:
+            raise ValueError("polynomial basis must be the same for all polynomials in a polynomial vector")
+        if maxDeg != p.Degree():
+            raise ValueError("polynomial degree must all be the same")
+    return PolynomialVector(polys, None if mapping is None else {int(k): [int(j) for j in v] for k, v in mapping.items()})
+
+
+def _check_vector(pv: PolynomialVector, max_slots: int, slots: int):
+    if pv.Mapping is None:
+        return
+    for i, js in pv.Mapping.items():
+        for j in js:
+            if i < len(pv.Value) and not 0 <= j < max_slots:
+                raise ValueError("mapping slot %d of polynomial %d out of range [0, %d)" % (j, i, max_slots))
+    if slots < max_slots:                         # the slot vectors have MaxSlots entries: Embed refuses them on fewer slots
+        raise ValueError("cannot Embed: ensure that #values (%d) <= slots (%d) <= maxCols (%d)" % (max_slots, slots, max_slots))
+
+
+def plan_vector(Q: Sequence[int], level: int, scale, pv: PolynomialVector, target_scale, levels_per_rescale: int = 1,
+                encoding_precision: int = 53, log_n: int = 0, log_slots: Optional[int] = None, roots1: Optional[Sequence[int]] = None) -> Program:
+    """The device program of Evaluate(ct, pv, targetScale) for a PolynomialVector. With a Mapping: every baby step in one PTLINCOMB and
+    program.plaintexts, the slot vectors to encode (values, level, scale). Without one: plan() of Value[0] (the reference's scalar
+    path), with the vector's odd / even flags. log_n: LogN of the ring (MaxSlots = 2^(LogN - 1)); log_slots: the ciphertext's LogSlots."""
+    if levels_per_rescale < 1:
+        raise ValueError("levels_per_rescale must be >= 1")
+    p0 = pv.Value[0]
+    if p0.basis not in (MONOMIAL, CHEBYSHEV):
+        raise ValueError("basis must be MONOMIAL or CHEBYSHEV")
+    if pv.Mapping is None and len(pv.Value) == 1:
+        return plan(Q, level, scale, p0.coeffs, p0.basis, target_scale, levels_per_rescale, encoding_precision, p0.odd, p0.even, roots1)
+    if log_n < 1:
+        raise ValueError("log_n must be the ring's LogN (>= 1), got %d" % log_n)
+    max_slots = 1 << (log_n - 1)
+    if pv.Mapping is not None:
+        if encoding_precision > 53:
+            raise ValueError("the polynomial-vector path encodes its slot vectors with the float64 encoder (EncodingPrecision <= 53); "
+                             "EncodingPrecision %d is not supported" % encoding_precision)
+        _check_vector(pv, max_slots, 1 << (log_n - 1 if log_slots is None else log_slots))
+    polys = [_Poly(_coeffs(q.coeffs), q.basis, q.odd, q.even) for q in pv.Value]
+    if polys[0].Degree() > 255:
+        raise ValueError("degree %d > 255 is not supported" % polys[0].Degree())
+    cplx = pv.Mapping is None and any(complex(c).imag != 0 for c in p0.coeffs)
+    if cplx and roots1 is None:
+        raise ValueError("complex coefficients need the ring's RootsForward[1]")
+    return _Planner(Q, levels_per_rescale, encoding_precision, roots1, max_slots).evaluate(level, Fraction(scale), polys[0], Fraction(target_scale),
+                                                                                          polys[1:], pv.Mapping)
+
+
+class PreparedVector:
+    """A vector program with its slot vectors encoded on the device: reusable for any batch of ciphertexts at the level and scale it was
+    planned for. pt: (n_pt, rows, N) int64 plaintext block, plaintext j's rows 0..pt_levels[j] written."""
+
+    def __init__(self, prog: Program, pt, pt_levels):
+        self.prog, self.pt, self.pt_levels = prog, pt, pt_levels
+        self.out_level, self.out_scale = prog.out_level, prog.out_scale
+
+    def structs(self, lpr: int):
+        cp = self.prog.to_c(lpr)
+        if self.pt is None:
+            return cp, None
+        return cp, self.prog.pt_weights_to_c(self.pt.data_ptr(), self.pt.shape[1] * self.pt.shape[2], self.pt_levels)
+
+
+def _pt_block(ctx: Context, prog: Program, encode_group, dtype):
+    """Allocates the plaintext block and encodes prog.plaintexts into it with one encode_group(values, level, scale, out_ptr, stride)
+    call per distinct (level, scale); returns (block, pt_levels) with the op's indices renumbered to the block's order."""
+    import torch
+    if not prog.plaintexts:
+        return None, []
+    groups: Dict[tuple, List[int]] = {}
+    for j, p in enumerate(prog.plaintexts):
+        groups.setdefault((p["level"], p["scale"]), []).append(j)
+    order = [j for g in groups.values() for j in g]
+    vals = [prog.values(j, dtype) for j in range(len(prog.plaintexts))]
+    new = {j: n for n, j in enumerate(order)}
+    rows = max(p["level"] for p in prog.plaintexts) + 1
+    N = ctx.N
+    block = torch.zeros((len(order), rows, N), dtype=torch.int64, device="cuda:%d" % ctx.device)
+    stride = rows * N
+    first = 0
+    for (lv, sc), js in groups.items():
+        encode_group(np.stack([vals[j] for j in js]), lv, sc, block.data_ptr() + 8 * first * stride, stride)
+        first += len(js)
+    o = [o for o in prog.ops if o["kind"] == PTLINCOMB][0]
+    o["index"] = [new[j] if j >= 0 else -1 for j in o["index"]]
+    prog.plaintexts = [prog.plaintexts[j] for j in order]
+    return block, [prog.plaintexts[n]["level"] for n in range(len(order))]
+
+
 class PolynomialEvaluator:
     """polynomial.Evaluator (circuits/ckks/polynomial) for one polynomial. encoding_precision = ckks.Parameters.EncodingPrecision()
     = max(53, log2(DefaultScale))."""
@@ -569,6 +836,55 @@ class PolynomialEvaluator:
         out = torch.empty(shape, dtype=torch.int64, device=ct.device)
         self.run(prog, ct, out, b)
         return out, prog.out_level, prog.out_scale
+
+    # ---- PolynomialVector (Evaluate with a Mapping) ----------------------------------------------------------------------
+    def plan_vector(self, level, scale, pv: PolynomialVector, target_scale, log_slots=None) -> Program:
+        cplx = pv.Mapping is None and any(complex(c).imag != 0 for c in pv.Value[0].coeffs)
+        return plan_vector(self.ctx.Q, level, scale, pv, target_scale, self.lpr, self.prec, self.ctx.logN, log_slots,
+                           self.roots1() if cplx else None)
+
+    def encode_plaintexts(self, prog: Program):
+        """The program's slot vectors, encoded with lgpu_ckks_encode (NTT, Embed at the plaintext's scale as float64, no host FFT): one
+        batched call per distinct (level, scale)."""
+        import torch
+        from .encoder import Encoder, ENC_NTT, _vp
+        if getattr(self, "_enc", None) is None:
+            self._enc = Encoder(self.ctx)
+        enc = self._enc
+        n = self.ctx.N // 2
+
+        def encode_group(values, level, scale, out_ptr, stride):
+            v = torch.from_numpy(values).to("cuda:%d" % self.ctx.device)
+            _lib.check(_lib.lib().lgpu_ckks_encode(self.ctx.h, _vp(v), n, self.ctx.logN - 1, float(scale), ENC_NTT, _vp(enc.rot_group),
+                                                   _vp(enc.roots), level, ctypes.c_void_p(out_ptr), -1, None, len(values), n, stride, 0,
+                                                   _stream()))
+        return _pt_block(self.ctx, prog, encode_group, np.complex128)
+
+    def PrepareVector(self, level, scale, pv: PolynomialVector, target_scale, log_slots=None) -> PreparedVector:
+        """Plans Evaluate(ct, pv, target_scale) for ciphertexts at (level, scale) and encodes its slot vectors on the device."""
+        prog = self.plan_vector(level, scale, pv, target_scale, log_slots)
+        pt, lv = self.encode_plaintexts(prog) if pv.Mapping is not None else (None, [])
+        return PreparedVector(prog, pt, lv)
+
+    def RunVector(self, prep: PreparedVector, ct):
+        """Runs a prepared plan on ct (batch, 2, level+1, N) or (2, level+1, N). Returns the output ciphertexts."""
+        import torch
+        b = ct.shape[0] if ct.dim() == 4 else 1
+        shape = (b, 2, prep.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prep.out_level + 1, self.ctx.N)
+        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
+        cp, vw = prep.structs(self.lpr)
+        if vw is None:
+            self.run(prep.prog, ct, out, b)
+        else:
+            _lib.check(_lib.lib().lgpu_ckks_polynomial_vector_evaluate(self.ctx.h, ct.shape[-2] - 1, _dptr(ct), b, ctypes.byref(cp),
+                                                                       ctypes.byref(vw), self.rlk.ref() if self.rlk is not None else None,
+                                                                       _dptr(out), _stream()))
+        return out
+
+    def EvaluateVector(self, ct, scale, pv: PolynomialVector, target_scale, log_slots=None):
+        """Evaluate(ct, PolynomialVector, targetScale) = PrepareVector + RunVector. Returns (ct_out, level, scale)."""
+        prep = self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, log_slots)
+        return self.RunVector(prep, ct), prep.out_level, prep.out_scale
 
     def run(self, prog: Program, ct, out, batch: int):
         cp = prog.to_c(self.lpr)

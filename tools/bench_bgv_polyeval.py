@@ -30,7 +30,7 @@ from lattigo_b200.params import PRESETS  # noqa: E402
 from bench_polyeval import gpu_info, timed, trim_pool  # noqa: E402
 
 
-def composed(ctx, bgv, ckks, rlk, prog, ct, t):
+def composed(ctx, bgv, ckks, rlk, prog, ct, t, extra=None):
     """The BGV program's op sequence through the existing entry points (see the module docstring). ct: (batch, 2, L+1, N)."""
     N, batch, Q = ctx.N, ct.shape[0], ctx.Q
     tmont = [(t << 128) % q for q in Q]             # tMontgomery = MForm(t 2^64 mod q)
@@ -93,7 +93,7 @@ def composed(ctx, bgv, ckks, rlk, prog, ct, t):
             y = torch.empty((batch, deg[src] + 1, lv + 1, N), dtype=torch.int64, device=ct.device)
             lb.div_by_last_modulus_many(ctx, lb.ring.RING_Q, rows(src) - 1, True, True, 1, x.reshape(-1, rows(src), N), y.view(-1, lv + 1, N))
             slots[o["dst"]] = ("il", y); deg[o["dst"]] = deg[src]
-        else:
+        elif k == PE.LINCOMB:
             L, terms, nt = lv, o["terms"], len(o["terms"])
             W = np.array(o["weights"], dtype=object).reshape(len(o["outs"]), nt + 1, L + 1, 2)
             for i_out, olv in enumerate(o["out_levels"]):
@@ -107,6 +107,8 @@ def composed(ctx, bgv, ckks, rlk, prog, ct, t):
                         ring(olv)._vec("MulScalarMontgomeryThenAdd", comp(sl, c, olv), None, acc[c],
                                        [(int(v) << 64) % Q[r] for r, v in enumerate(w)])
                 slots[o["outs"][i_out]] = ("pc", acc); deg[o["outs"][i_out]] = 1
+        else:                                            # an op of another program kind: extra(op, comp, slots, deg)
+            extra(o, comp, slots, deg)
         for sl in [s_ for s_, j in last.items() if j == i and s_ != 0 and s_ != prog.out_slot]:
             slots.pop(sl, None)
             for key in [key for key in cache if key[0] == sl]:

@@ -43,7 +43,7 @@ def gpu_info():
     return name, float(limit)
 
 
-def composed(ctx, ckks, rlk, prog, ct, lpr):
+def composed(ctx, ckks, rlk, prog, ct, lpr, extra=None):
     """The program's op sequence through the existing entry points (see the module docstring). ct: (batch, 2, L+1, N)."""
     from lattigo_b200.ring import SubRing
     N, batch = ctx.N, ct.shape[0]
@@ -144,7 +144,7 @@ def composed(ctx, ckks, rlk, prog, ct, lpr):
                 d.append(y)
             if not continue_after:
                 slots[o["dst"]] = ("pc", d); deg[o["dst"]] = deg[src]
-        else:
+        elif k == PE.LINCOMB:
             L, terms, nt = lv, o["terms"], len(o["terms"])
             W = np.array(o["weights"], dtype=object).reshape(len(o["outs"]), nt + 1, L + 1, 2)
             order = sorted(range(len(o["outs"])), key=lambda j: -o["out_levels"][j])
@@ -163,6 +163,8 @@ def composed(ctx, ckks, rlk, prog, ct, lpr):
                 if n_done + 1 == len(order) or o["out_levels"][order[n_done + 1]] != olv:
                     for key in [key for key in cache if key[2] == olv and key[0] in terms]:      # copies made for this level
                         del cache[key]
+        else:                                            # an op of another program kind: extra(op, comp, slots, deg)
+            extra(o, comp, slots, deg)
         for sl in [s_ for s_, j in last.items() if j == i and s_ != 0 and s_ != prog.out_slot]:
             slots.pop(sl, None)
             for key in [key for key in cache if key[0] == sl]:
