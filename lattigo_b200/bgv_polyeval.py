@@ -22,9 +22,9 @@ from typing import Sequence
 import numpy as np
 
 from . import _lib
-from .polyeval import (CHEBYSHEV, MONOMIAL, MULRELIN, RESCALE, TENSOR, PolynomialVector, PreparedVector, Program, _check_vector, _Lin,
-                       _Planner, _Poly, _pt_block, _Sim, _Sym, _VLin)
-from .ring import _dptr, _stream
+from .polyeval import (CHEBYSHEV, MONOMIAL, MULRELIN, RESCALE, TENSOR, Polynomial, PolynomialVector, PreparedVector, Program, _check_vector,
+                       _Evaluator, _Lin, _Planner, _Poly, _pt_block, _Sim, _Sym, _VLin)
+from .ring import _stream
 
 U64_MAX = (1 << 64) - 1
 
@@ -218,45 +218,29 @@ def plan(Q: Sequence[int], t: int, level: int, scale: int, coeffs: Sequence[int]
          odd: bool = True, even: bool = True, basis: int = MONOMIAL) -> Program:
     """The device program of Evaluate(ct, bignum.NewPolynomial(Monomial, coeffs, nil) with IsOdd = odd, IsEven = even, targetScale) for a
     ciphertext at `level` with rlwe.Scale `scale` (Mod = t); scale_invariant is the evaluator's ScaleInvariant (InvariantTensoring)."""
-    if basis == CHEBYSHEV:
-        raise ValueError("the Chebyshev basis is not supported for BGV polynomial evaluation (uint64 coefficients); use the monomial basis")
-    if basis != MONOMIAL:
-        raise ValueError("basis must be MONOMIAL")
-    coeffs = [int(c) for c in coeffs]
-    if any(c < 0 or c > U64_MAX for c in coeffs):
-        raise ValueError("coefficients must be uint64")
-    t = int(t)
-    for name, s in (("scale", scale), ("target_scale", target_scale)):
-        if not 1 <= int(s) < t:
-            raise ValueError("%s must be an integer in [1, t)" % name)
-    p = _Poly(list(coeffs), MONOMIAL, odd, even)
-    if p.Degree() > 255:
-        raise ValueError("degree %d > 255 is not supported" % p.Degree())
-    return _BGVPlanner(Q, t, bool(scale_invariant)).evaluate(level, int(scale), p, int(target_scale))
+    return plan_vector(Q, t, level, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale, scale_invariant)
 
 
 def plan_vector(Q: Sequence[int], t: int, level: int, scale: int, pv: PolynomialVector, target_scale: int, scale_invariant: bool = False,
                 max_slots: int = 0) -> Program:
     """The device program of Evaluate(ct, pv, targetScale) for a PolynomialVector of monomial-basis uint64 polynomials: with a Mapping,
-    every baby step in one PTLINCOMB plus program.plaintexts (slot vectors Encode'd at (level, scale), scale mod t); without one,
-    plan() of Value[0]. max_slots: MaxSlots of the parameters (the length of the slot vectors)."""
+    every baby step in one PTLINCOMB plus program.plaintexts (slot vectors Encode'd at (level, scale), scale mod t); without one, the
+    scalar program of Value[0]. max_slots: MaxSlots of the parameters (the length of the slot vectors), needed with a Mapping."""
     p0 = pv.Value[0]
-    if pv.Mapping is None and len(pv.Value) == 1:
-        return plan(Q, t, level, scale, p0.coeffs, target_scale, scale_invariant, p0.odd, p0.even, p0.basis)
     if p0.basis == CHEBYSHEV:
         raise ValueError("the Chebyshev basis is not supported for BGV polynomial evaluation (uint64 coefficients); use the monomial basis")
     if p0.basis != MONOMIAL:
         raise ValueError("basis must be MONOMIAL")
-    t = int(t)
-    for name, s in (("scale", scale), ("target_scale", target_scale)):
-        if not 1 <= int(s) < t:
-            raise ValueError("%s must be an integer in [1, t)" % name)
     polys = []
     for q in pv.Value:
         coeffs = [int(c) for c in q.coeffs]
         if any(c < 0 or c > U64_MAX for c in coeffs):
             raise ValueError("coefficients must be uint64")
         polys.append(_Poly(coeffs, MONOMIAL, q.odd, q.even))
+    t = int(t)
+    for name, s in (("scale", scale), ("target_scale", target_scale)):
+        if not 1 <= int(s) < t:
+            raise ValueError("%s must be an integer in [1, t)" % name)
     if polys[0].Degree() > 255:
         raise ValueError("degree %d > 255 is not supported" % polys[0].Degree())
     if pv.Mapping is not None:
@@ -266,27 +250,21 @@ def plan_vector(Q: Sequence[int], t: int, level: int, scale: int, pv: Polynomial
     return _BGVPlanner(Q, t, bool(scale_invariant), max_slots).evaluate(level, int(scale), polys[0], int(target_scale), polys[1:], pv.Mapping)
 
 
-class BGVPolynomialEvaluator:
+class BGVPolynomialEvaluator(_Evaluator):
     """polynomial.Evaluator (circuits/bgv/polynomial) over a BGVEvaluator: InvariantTensoring = bgv_evaluator.ScaleInvariant."""
 
     def __init__(self, bgv_evaluator):
         self.ev = bgv_evaluator
         self.ctx = bgv_evaluator.ctx
         self.InvariantTensoring = bgv_evaluator.ScaleInvariant
+        self.lpr = 1                              # Rescale drops one modulus
 
     def plan(self, level, scale, coeffs, target_scale, odd=True, even=True, basis=MONOMIAL) -> Program:
-        return plan(self.ctx.Q, self.ev.t, level, scale, coeffs, target_scale, self.InvariantTensoring, odd, even, basis)
+        return self.plan_vector(level, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale)
 
     def Evaluate(self, ct, scale, coeffs, target_scale, odd=True, even=True, basis=MONOMIAL):
         """ct: (batch, 2, level+1, N) or (2, level+1, N) int64 CUDA tensor, NTT domain. Returns (ct_out, level, scale)."""
-        import torch
-        level = ct.shape[-2] - 1
-        prog = self.plan(level, scale, coeffs, target_scale, odd, even, basis)
-        b = ct.shape[0] if ct.dim() == 4 else 1
-        shape = (b, 2, prog.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prog.out_level + 1, self.ctx.N)
-        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
-        self.run(prog, ct, out, b)
-        return out, prog.out_level, prog.out_scale
+        return self.EvaluateVector(ct, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale, None)
 
     # ---- PolynomialVector (Evaluate with a Mapping) ----------------------------------------------------------------------
     def plan_vector(self, level, scale, pv: PolynomialVector, target_scale) -> Program:
@@ -309,34 +287,15 @@ class BGVPolynomialEvaluator:
 
     def PrepareVector(self, level, scale, pv: PolynomialVector, target_scale, encoder) -> PreparedVector:
         """Plans Evaluate(ct, pv, target_scale) for ciphertexts at (level, scale) and encodes its slot vectors on the device."""
-        prog = self.plan_vector(level, scale, pv, target_scale)
-        pt, lv = self.encode_plaintexts(prog, encoder) if pv.Mapping is not None else (None, [])
-        return PreparedVector(prog, pt, lv)
-
-    def RunVector(self, prep: PreparedVector, ct):
-        """Runs a prepared plan on ct (batch, 2, level+1, N) or (2, level+1, N). Returns the output ciphertexts."""
-        import torch
-        b = ct.shape[0] if ct.dim() == 4 else 1
-        shape = (b, 2, prep.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prep.out_level + 1, self.ctx.N)
-        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
-        cp, vw = prep.structs(1)
-        if vw is None:
-            self.run(prep.prog, ct, out, b)
-        else:
-            rlk = self.ev.rlk
-            _lib.check(_lib.lib().lgpu_bgv_polynomial_vector_evaluate(self.ev.h, ct.shape[-2] - 1, _dptr(ct), b, ctypes.byref(cp), ctypes.byref(vw),
-                                                                      rlk.ref() if rlk is not None else None, 1 if self.InvariantTensoring else 0,
-                                                                      _dptr(out), _stream()))
-        return out
+        return self._prepare(self.plan_vector(level, scale, pv, target_scale), pv, encoder)
 
     def EvaluateVector(self, ct, scale, pv: PolynomialVector, target_scale, encoder):
         """Evaluate(ct, PolynomialVector, targetScale) = PrepareVector + RunVector. Returns (ct_out, level, scale)."""
-        prep = self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, encoder)
-        return self.RunVector(prep, ct), prep.out_level, prep.out_scale
+        return self._evaluate(ct, self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, encoder))
 
-    def run(self, prog: Program, ct, out, batch: int):
-        cp = prog.to_c(1)
-        rlk = self.ev.rlk
-        _lib.check(_lib.lib().lgpu_bgv_polynomial_evaluate(self.ev.h, ct.shape[-2] - 1, _dptr(ct), batch, ctypes.byref(cp),
-                                                           rlk.ref() if rlk is not None else None, 1 if self.InvariantTensoring else 0,
-                                                           _dptr(out), _stream()))
+    def _call(self, level, ct, batch, prog, pts, out):
+        rlk = self.ev.rlk.ref() if self.ev.rlk is not None else None
+        si = 1 if self.InvariantTensoring else 0
+        if pts is None:
+            return _lib.lib().lgpu_bgv_polynomial_evaluate(self.ev.h, level, ct, batch, prog, rlk, si, out, _stream())
+        return _lib.lib().lgpu_bgv_polynomial_vector_evaluate(self.ev.h, level, ct, batch, prog, pts, rlk, si, out, _stream())

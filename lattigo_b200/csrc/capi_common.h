@@ -29,9 +29,11 @@ struct lgpu_ctx {
     } while (0)
 // every device entry point opens an NVTX range named after itself (visible in nsys / ncu --nvtx; a no-op without a tool attached), so that a
 // trace of the Go application shows which ring / evaluator method each group of kernels belongs to
-#define REQUIRE_DEVICE(ctx)                                                                                                      \
+#define REQUIRE_DEVICE(ctx) REQUIRE_DEVICE_AS(ctx, __func__)
+// the same in a helper that runs on behalf of the entry point `name`
+#define REQUIRE_DEVICE_AS(ctx, name)                                                                                             \
     REQUIRE((ctx) && (ctx)->c.device >= 0, "this context was created host-only (device < 0): no device execution");             \
-    lgpu::NvtxRange lgpu_nvtx_range_(__func__)
+    lgpu::NvtxRange lgpu_nvtx_range_(name)
 // the key-switch family moves 128 bits per access: polynomial blocks must be 16-byte aligned with even strides
 #define AL(p) ((reinterpret_cast<uintptr_t>(p) & 15u) == 0)
 #define REQUIRE_ALIGNED(cond) REQUIRE(cond, "polynomial buffers and evaluation keys must be 16-byte aligned with even strides (words)")

@@ -243,7 +243,7 @@ struct Plan {           // what validation derives from the program
 };
 
 // vw: the plaintext table of the vector entry points; null for the scalar ones, where PTLINCOMB stays an unknown op
-int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, const lgpu_poly_pt_weights* vw = nullptr) {
+int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, const lgpu_poly_pt_weights* vw) {
     REQUIRE(pg && pg->n_ops >= 1 && pg->ops, "empty polynomial program");
     REQUIRE(pg->n_slots >= 2 && pg->n_slots <= (1 << 16), "program slot count out of range");
     REQUIRE(pg->levels_per_rescale >= 1, "levels_per_rescale must be >= 1");
@@ -259,60 +259,37 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, con
         }
         return true;
     };
+    // single assignment: slot d is written once, and never slot 0 (the input)
+    auto write = [&](int d, int deg, int lv) {
+        REQUIRE(slot_ok(d) && pl.level[d] < 0 && d != 0, "program writes a slot twice (or slot 0)");
+        pl.deg[d] = deg; pl.level[d] = lv;
+        return 0;
+    };
+    // what LINCOMB and PTLINCOMB (op i, named `name` in the messages) share: output and term counts, the arrays, output levels whose
+    // maximum is the op's level, degree-1 terms
+    auto lin_shape = [&](const lgpu_poly_op& o, int i, const std::string& name) {
+        const bool lin = o.kind == LGPU_POLY_LINCOMB;
+        REQUIRE(o.n_out >= 1 && o.n_out <= kPolyMaxOut, name + " output count out of range");
+        REQUIRE(o.n_terms >= 0 && o.n_terms <= kPolyMaxTerms, name + " term count out of range (at most LGPU_POLY_MAX_TERMS)");
+        REQUIRE(o.outs && o.out_levels && (!lin || o.weights) && (o.n_terms == 0 || o.terms),
+                name + (lin ? " needs outs, out_levels, terms and weights" : " needs outs, out_levels and terms"));
+        int mx = -1;
+        for (int k = 0; k < o.n_out; k++) {
+            REQUIRE(o.out_levels[k] >= 0 && o.out_levels[k] <= o.level, name + " output level out of range");
+            mx = std::max(mx, o.out_levels[k]);
+        }
+        REQUIRE(mx == o.level, name + " level must be the maximum of its output levels");
+        for (int k = 0; k < o.n_terms; k++) {
+            REQUIRE(readable(o.terms[k]), "program reads a slot before it is written");
+            REQUIRE(pl.deg[o.terms[k]] == 1, name + " terms must have degree 1");
+            pl.last_use[o.terms[k]] = i;
+        }
+        return 0;
+    };
     int n_pt_ops = 0;
     for (int i = 0; i < pg->n_ops; i++) {
         const lgpu_poly_op& o = pg->ops[i];
         REQUIRE(o.level >= 0 && o.level <= level, "program op level out of range");
-        if (o.kind == LGPU_POLY_PTLINCOMB && vw) {
-            REQUIRE(++n_pt_ops == 1, "a vector program has exactly one PTLINCOMB op");
-            REQUIRE(o.n_out >= 1 && o.n_out <= kPolyMaxOut, "PTLINCOMB output count out of range");
-            REQUIRE(o.n_terms >= 0 && o.n_terms <= kPolyMaxTerms, "PTLINCOMB term count out of range (at most LGPU_POLY_MAX_TERMS)");
-            REQUIRE(o.outs && o.out_levels && (o.n_terms == 0 || o.terms), "PTLINCOMB needs outs, out_levels and terms");
-            REQUIRE(vw->n_pt >= 1 && vw->n_pt <= (1 << 20), "plaintext count out of range");
-            REQUIRE(vw->pt && vw->pt_levels && vw->index && vw->scalars, "null plaintext table");
-            REQUIRE_ALIGNED(AL(vw->pt) && vw->pt_stride % 2 == 0);
-            for (int j = 0; j < vw->n_pt; j++) REQUIRE(vw->pt_levels[j] >= 0 && vw->pt_levels[j] < c.nQ, "plaintext level out of range");
-            int mx = -1;
-            for (int k = 0; k < o.n_out; k++) {
-                REQUIRE(o.out_levels[k] >= 0 && o.out_levels[k] <= o.level, "PTLINCOMB output level out of range");
-                mx = std::max(mx, o.out_levels[k]);
-            }
-            REQUIRE(mx == o.level, "PTLINCOMB level must be the maximum of its output levels");
-            int ptmax = 0;
-            for (int j = 0; j < vw->n_pt; j++) ptmax = std::max(ptmax, vw->pt_levels[j]);
-            REQUIRE(vw->pt_stride >= (size_t)(ptmax + 1) * c.N, "plaintext stride below the rows of its plaintexts");
-            for (int t = 0; t < o.n_terms; t++) {
-                REQUIRE(readable(o.terms[t]), "program reads a slot before it is written");
-                REQUIRE(pl.deg[o.terms[t]] == 1, "PTLINCOMB terms must have degree 1");
-                pl.last_use[o.terms[t]] = i;
-            }
-            const int K = o.n_terms + 1, R = o.level + 1;
-            for (int k = 0; k < o.n_out; k++)
-                for (int t = 0; t < K; t++) {
-                    const int id = vw->index[k * K + t];
-                    REQUIRE(id >= -1 && id < vw->n_pt, "plaintext index out of range");
-                    if (id < 0) continue;
-                    REQUIRE(vw->pt_levels[id] >= o.out_levels[k], "PTLINCOMB output uses a plaintext below its level");
-                    REQUIRE(t == o.n_terms || pl.level[o.terms[t]] >= o.out_levels[k], "PTLINCOMB output uses a term below its level");
-                }
-            REQUIRE(w_ok(vw->scalars, (size_t)o.n_out * K * R, R, 1), "PTLINCOMB scalar not below its modulus");
-            for (int k = 0; k < o.n_out; k++) {
-                const int d = o.outs[k];
-                REQUIRE(slot_ok(d) && pl.level[d] < 0 && d != 0, "program writes a slot twice (or slot 0)");
-                pl.deg[d] = 1; pl.level[d] = o.out_levels[k];
-            }
-            // device layout: [limb][out][term] Montgomery factors (s 2^128 for a term, s 2^64 for the constant), then [out][term] indices
-            std::vector<u64>& w = pl.w[i];
-            w.resize((size_t)R * o.n_out * K + (size_t)o.n_out * K);
-            for (int r = 0; r < R; r++)
-                for (int k = 0; k < o.n_out; k++)
-                    for (int t = 0; t < K; t++) {
-                        const u64 v = h_mform(vw->scalars[((size_t)k * K + t) * R + r], c.Q[r]);
-                        w[((size_t)r * o.n_out + k) * K + t] = t < o.n_terms ? h_mform(v, c.Q[r]) : v;
-                    }
-            for (int k = 0; k < o.n_out * K; k++) w[(size_t)R * o.n_out * K + k] = vw->index[k] < 0 ? ~0ull : (u64)vw->index[k];
-            continue;
-        }
         switch (o.kind) {
         case LGPU_POLY_MULRELIN:
         case LGPU_POLY_TENSOR: {
@@ -330,8 +307,7 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, con
                 std::vector<u64>& w = pl.w[i];
                 for (int k = 0; k < 2 * (o.level + 1); k++) w.push_back(h_mform(o.weights[k], c.Q[k % (o.level + 1)]));
             }
-            REQUIRE(slot_ok(o.dst) && pl.level[o.dst] < 0 && o.dst != 0, "program writes a slot twice (or slot 0)");
-            pl.deg[o.dst] = o.kind == LGPU_POLY_MULRELIN ? 1 : 2; pl.level[o.dst] = o.level;
+            if (write(o.dst, o.kind == LGPU_POLY_MULRELIN ? 1 : 2, o.level)) return -1;
             pl.last_use[o.src0] = pl.last_use[o.src1] = i;
             if (o.kind == LGPU_POLY_TENSOR && o.addend >= 0) pl.last_use[o.addend] = i;
             break;
@@ -345,26 +321,12 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, con
             } else {
                 REQUIRE(o.level == pl.level[o.src0] - pg->levels_per_rescale, "cannot Rescale: RESCALE level must be its operand's minus levels_per_rescale");
             }
-            REQUIRE(slot_ok(o.dst) && pl.level[o.dst] < 0 && o.dst != 0, "program writes a slot twice (or slot 0)");
-            pl.deg[o.dst] = o.kind == LGPU_POLY_RELIN ? 1 : pl.deg[o.src0]; pl.level[o.dst] = o.level;
+            if (write(o.dst, o.kind == LGPU_POLY_RELIN ? 1 : pl.deg[o.src0], o.level)) return -1;
             pl.last_use[o.src0] = i;
             break;
         }
         case LGPU_POLY_LINCOMB: {
-            REQUIRE(o.n_out >= 1 && o.n_out <= kPolyMaxOut, "LINCOMB output count out of range");
-            REQUIRE(o.n_terms >= 0 && o.n_terms <= kPolyMaxTerms, "LINCOMB term count out of range (at most LGPU_POLY_MAX_TERMS)");
-            REQUIRE(o.outs && o.out_levels && o.weights && (o.n_terms == 0 || o.terms), "LINCOMB needs outs, out_levels, terms and weights");
-            int mx = -1;
-            for (int k = 0; k < o.n_out; k++) {
-                REQUIRE(o.out_levels[k] >= 0 && o.out_levels[k] <= o.level, "LINCOMB output level out of range");
-                mx = std::max(mx, o.out_levels[k]);
-            }
-            REQUIRE(mx == o.level, "LINCOMB level must be the maximum of its output levels");
-            for (int k = 0; k < o.n_terms; k++) {
-                REQUIRE(readable(o.terms[k]), "program reads a slot before it is written");
-                REQUIRE(pl.deg[o.terms[k]] == 1, "LINCOMB terms must have degree 1");
-                pl.last_use[o.terms[k]] = i;
-            }
+            if (lin_shape(o, i, "LINCOMB")) return -1;
             const int K = o.n_terms + 1, R = o.level + 1;
             REQUIRE(w_ok(o.weights, (size_t)o.n_out * K * R * 2, R, 2), "LINCOMB weight not below its modulus");
             for (int k = 0; k < o.n_out; k++)            // an output may not use a term above the term's level
@@ -372,11 +334,8 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, con
                     for (int r = pl.level[o.terms[t]] + 1; r <= o.out_levels[k]; r++)
                         REQUIRE(o.weights[(((size_t)k * K + t) * R + r) * 2] == 0 && o.weights[(((size_t)k * K + t) * R + r) * 2 + 1] == 0,
                                 "LINCOMB output uses a term above the term's level");
-            for (int k = 0; k < o.n_out; k++) {
-                const int d = o.outs[k];
-                REQUIRE(slot_ok(d) && pl.level[d] < 0 && d != 0, "program writes a slot twice (or slot 0)");
-                pl.deg[d] = 1; pl.level[d] = o.out_levels[k];
-            }
+            for (int k = 0; k < o.n_out; k++)
+                if (write(o.outs[k], 1, o.out_levels[k])) return -1;
             // device layout [limb][out][term][half], Montgomery form for the terms, the constant as is
             std::vector<u64>& w = pl.w[i];
             w.resize((size_t)R * o.n_out * K * 2);
@@ -387,6 +346,43 @@ int validate(const Ctx& c, int level, const lgpu_poly_program* pg, Plan& pl, con
                             const u64 v = o.weights[(((size_t)k * K + t) * R + r) * 2 + h];
                             w[(((size_t)r * o.n_out + k) * K + t) * 2 + h] = t < o.n_terms ? h_mform(v, c.Q[r]) : v;
                         }
+            break;
+        }
+        case LGPU_POLY_PTLINCOMB: {
+            REQUIRE(vw, "unknown polynomial program op");          // to the scalar entry points
+            REQUIRE(++n_pt_ops == 1, "a vector program has exactly one PTLINCOMB op");
+            if (lin_shape(o, i, "PTLINCOMB")) return -1;
+            REQUIRE(vw->n_pt >= 1 && vw->n_pt <= (1 << 20), "plaintext count out of range");
+            REQUIRE(vw->pt && vw->pt_levels && vw->index && vw->scalars, "null plaintext table");
+            REQUIRE_ALIGNED(AL(vw->pt) && vw->pt_stride % 2 == 0);
+            int ptmax = 0;
+            for (int j = 0; j < vw->n_pt; j++) {
+                REQUIRE(vw->pt_levels[j] >= 0 && vw->pt_levels[j] < c.nQ, "plaintext level out of range");
+                ptmax = std::max(ptmax, vw->pt_levels[j]);
+            }
+            REQUIRE(vw->pt_stride >= (size_t)(ptmax + 1) * c.N, "plaintext stride below the rows of its plaintexts");
+            const int K = o.n_terms + 1, R = o.level + 1;
+            for (int k = 0; k < o.n_out; k++)
+                for (int t = 0; t < K; t++) {
+                    const int id = vw->index[k * K + t];
+                    REQUIRE(id >= -1 && id < vw->n_pt, "plaintext index out of range");
+                    if (id < 0) continue;
+                    REQUIRE(vw->pt_levels[id] >= o.out_levels[k], "PTLINCOMB output uses a plaintext below its level");
+                    REQUIRE(t == o.n_terms || pl.level[o.terms[t]] >= o.out_levels[k], "PTLINCOMB output uses a term below its level");
+                }
+            REQUIRE(w_ok(vw->scalars, (size_t)o.n_out * K * R, R, 1), "PTLINCOMB scalar not below its modulus");
+            for (int k = 0; k < o.n_out; k++)
+                if (write(o.outs[k], 1, o.out_levels[k])) return -1;
+            // device layout: [limb][out][term] Montgomery factors (s 2^128 for a term, s 2^64 for the constant), then [out][term] indices
+            std::vector<u64>& w = pl.w[i];
+            w.resize((size_t)R * o.n_out * K + (size_t)o.n_out * K);
+            for (int r = 0; r < R; r++)
+                for (int k = 0; k < o.n_out; k++)
+                    for (int t = 0; t < K; t++) {
+                        const u64 v = h_mform(vw->scalars[((size_t)k * K + t) * R + r], c.Q[r]);
+                        w[((size_t)r * o.n_out + k) * K + t] = t < o.n_terms ? h_mform(v, c.Q[r]) : v;
+                    }
+            for (int k = 0; k < o.n_out * K; k++) w[(size_t)R * o.n_out * K + k] = vw->index[k] < 0 ? ~0ull : (u64)vw->index[k];
             break;
         }
         default:
@@ -415,13 +411,15 @@ struct Runner {
     const BgvState* bgv = nullptr;        // BGV / BFV: the evaluator state; null for CKKS
     bool si = false;                      // BFV: scale-invariant tensoring
     const lgpu_poly_pt_weights* vw = nullptr;   // the vector entry points' plaintexts
+    u64* out_chunk = nullptr;             // the sub-batch's output ciphertexts: the program's output slot is written there
 
     size_t cs(int i) const { return (size_t)(s[i].level + 1) * c->N; }
     size_t bs(int i) const { return (size_t)(s[i].deg + 1) * cs(i); }
 
-    int make(int i, u64* out_chunk) {
+    // slot i: out_chunk if it is the program's output, else a new sub-batch block
+    int make(int i) {
         s[i].deg = pl.deg[i]; s[i].level = pl.level[i];
-        if (out_chunk) { s[i].p = out_chunk; return 0; }
+        if (i == pg->out_slot) { s[i].p = out_chunk; return 0; }
         LGPU_CUDA_OK(cudaMallocAsync((void**)&s[i].p, (size_t)nb * bs(i) * 8, st));
         s[i].owned = true;
         return 0;
@@ -490,9 +488,24 @@ struct Runner {
         return 0;
     }
 
+    // the term and output arrays of a LINCOMB / PTLINCOMB launch; makes the output slots
+    template <class P>
+    int lin_io(const lgpu_poly_op& o, P& p) {
+        for (int k = 0; k < o.n_terms; k++) {
+            const int t = o.terms[k];
+            p.in[k] = s[t].p; p.in_cs[k] = (unsigned)cs(t); p.in_bs[k] = (unsigned)bs(t); p.in_level[k] = s[t].level;
+        }
+        for (int k = 0; k < o.n_out; k++) {
+            const int d = o.outs[k];
+            if (make(d)) return -1;
+            p.out[k] = s[d].p; p.out_cs[k] = (unsigned)cs(d); p.out_bs[k] = (unsigned)bs(d); p.out_level[k] = o.out_levels[k];
+        }
+        return 0;
+    }
+
     // PTLINCOMB: batch tiles of BT = min(8, nb) rounded up to a power of two (1, 2, 4, 8), so a sub-batch of up to 8 ciphertexts is
     // one tile and reads each plaintext word once; larger sub-batches read it once per 8 ciphertexts
-    int pt_lincomb(int i, u64* out_chunk) {
+    int pt_lincomb(int i) {
         const lgpu_poly_op& o = pg->ops[i];
         const size_t N = c->N;
         const int K1 = o.n_terms + 1;
@@ -500,15 +513,7 @@ struct Runner {
         p.limbs = c->d_limbs; p.w = d_w + w_off[i]; p.idx = p.w + (size_t)(o.level + 1) * o.n_out * K1;
         p.pt = (const u64*)vw->pt; p.pt_stride = vw->pt_stride;
         p.n_out = o.n_out; p.n_terms = o.n_terms; p.n = c->N; p.nb = nb;
-        for (int k = 0; k < o.n_terms; k++) {
-            p.in[k] = s[o.terms[k]].p; p.in_cs[k] = (unsigned)cs(o.terms[k]); p.in_bs[k] = (unsigned)bs(o.terms[k]);
-            p.in_level[k] = s[o.terms[k]].level;
-        }
-        for (int k = 0; k < o.n_out; k++) {
-            const int d = o.outs[k];
-            if (make(d, d == pg->out_slot ? out_chunk : nullptr)) return -1;
-            p.out[k] = s[d].p; p.out_cs[k] = (unsigned)cs(d); p.out_bs[k] = (unsigned)bs(d); p.out_level[k] = o.out_levels[k];
-        }
+        if (lin_io(o, p)) return -1;
         const int bt = nb > 4 ? 8 : nb > 2 ? 4 : nb, cj = 256 / bt, tiles = (nb + bt - 1) / bt;
         // bytes: powers once per entry, plaintexts once per tile (every (output, term) pair with a plaintext), outputs once
         double pts = 0;
@@ -527,24 +532,24 @@ struct Runner {
         return 0;
     }
 
-    int op(int i, u64* out_chunk) {
+    int op(int i) {
         const lgpu_poly_op& o = pg->ops[i];
         const size_t N = c->N;
         switch (o.kind) {
         case LGPU_POLY_MULRELIN:
-            if (make(o.dst, o.dst == pg->out_slot ? out_chunk : nullptr)) return -1;
+            if (make(o.dst)) return -1;
             return mulrelin(o);
         case LGPU_POLY_TENSOR:
-            if (make(o.dst, nullptr)) return -1;
+            if (make(o.dst)) return -1;
             return tensor_op(i);
         case LGPU_POLY_RELIN: {
-            if (make(o.dst, o.dst == pg->out_slot ? out_chunk : nullptr)) return -1;
+            if (make(o.dst)) return -1;
             const int a = o.src0, d = o.dst;
             return evaluator_relinearize(c, o.level, CSpan{s[a].p, N, bs(a)}, CSpan{s[a].p + cs(a), N, bs(a)}, CSpan{s[a].p + 2 * cs(a), N, bs(a)}, rlk,
                                          Span{s[d].p, N, bs(d)}, Span{s[d].p + cs(d), N, bs(d)}, nb, st);
         }
         case LGPU_POLY_RESCALE: {
-            if (make(o.dst, o.dst == pg->out_slot ? out_chunk : nullptr)) return -1;
+            if (make(o.dst)) return -1;
             const int a = o.src0, d = o.dst;
             // every polynomial of the sub-batch is one (level+1) x N block at a constant stride: one call for all of them
             return div_by_last_modulus_many(c, LGPU_RING_Q, s[a].level, true, true, pg->levels_per_rescale, CSpan{s[a].p, N, cs(a)}, Span{s[d].p, N, cs(d)},
@@ -553,15 +558,7 @@ struct Runner {
         case LGPU_POLY_LINCOMB: {
             LincombParams p;
             p.limbs = c->d_limbs; p.w = d_w + w_off[i]; p.n_out = o.n_out; p.n_terms = o.n_terms; p.n = c->N;
-            for (int k = 0; k < o.n_terms; k++) {
-                p.in[k] = s[o.terms[k]].p; p.in_cs[k] = (unsigned)cs(o.terms[k]); p.in_bs[k] = (unsigned)bs(o.terms[k]);
-                p.in_level[k] = s[o.terms[k]].level;
-            }
-            for (int k = 0; k < o.n_out; k++) {
-                const int d = o.outs[k];
-                if (make(d, d == pg->out_slot ? out_chunk : nullptr)) return -1;
-                p.out[k] = s[d].p; p.out_cs[k] = (unsigned)cs(d); p.out_bs[k] = (unsigned)bs(d); p.out_level[k] = o.out_levels[k];
-            }
+            if (lin_io(o, p)) return -1;
             const size_t smem = (size_t)o.n_out * (o.n_terms + 1) * 2 * 8;
             ProfScope ps(LGPU_KCLASS_VECOP, st, 8.0 * N * (o.level + 1) * nb * 2 * (o.n_terms + o.n_out), 1);
             poly_lincomb_kernel<<<dim3((c->N + 255) / 256, (unsigned)(o.level + 1), (unsigned)nb), 256, smem, st>>>(p);
@@ -569,7 +566,7 @@ struct Runner {
             return 0;
         }
         case LGPU_POLY_PTLINCOMB:
-            return pt_lincomb(i, out_chunk);
+            return pt_lincomb(i);
         }
         return 0;
     }
@@ -603,7 +600,7 @@ int program_rlk(const Ctx& c, const lgpu_poly_program* prog, const lgpu_gadget_c
 
 // runs a validated program over the batch, one batch_chunk() sub-batch at a time
 int run_program(const Ctx& c, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog, const Plan& pl, const GadgetCt& g,
-                const BgvState* bgv, bool si, uint64_t* ct_out, cudaStream_t st, const lgpu_poly_pt_weights* vw = nullptr) {
+                const BgvState* bgv, bool si, uint64_t* ct_out, cudaStream_t st, const lgpu_poly_pt_weights* vw) {
     std::vector<u64> hw;
     std::vector<size_t> off(prog->n_ops, 0);
     for (int i = 0; i < prog->n_ops; i++) { off[i] = hw.size(); hw.insert(hw.end(), pl.w[i].begin(), pl.w[i].end()); }
@@ -617,16 +614,42 @@ int run_program(const Ctx& c, int level, const uint64_t* ct_in, int batch, const
     const int ch = batch_chunk();
     for (int k = 0; k < batch; k += ch) {
         const int nb = std::min(ch, batch - k);
-        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off, bgv, si, vw};
+        Runner R{&c, prog, pl, g, st, nb, std::vector<Slot>(prog->n_slots), dw.p, off, bgv, si, vw, (u64*)ct_out + (size_t)k * co};
         R.s[0].p = (u64*)ct_in + (size_t)k * ci; R.s[0].deg = 1; R.s[0].level = level;
-        u64* out = (u64*)ct_out + (size_t)k * co;
         for (int i = 0; i < prog->n_ops; i++) {
-            if (R.op(i, out)) return -1;
+            if (R.op(i)) return -1;
             for (int sl = 1; sl < prog->n_slots; sl++)
                 if (pl.last_use[sl] == i && sl != prog->out_slot) R.release(sl);
         }
     }
     return 0;
+}
+
+// the four entry points after their handle checks (fn: the entry point's name, for its NVTX range). bgv: the BGV / BFV evaluator
+// state, null for CKKS; vector: a vector entry point, whose plaintext table vw may not be null (vw is null for the scalar ones)
+int evaluate(const char* fn, lgpu_ctx* ctx, const BgvState* bgv, int scale_invariant, int level, const uint64_t* ct_in, int batch,
+             const lgpu_poly_program* prog, bool vector, const lgpu_poly_pt_weights* vw, const lgpu_gadget_ct* rlk, uint64_t* ct_out,
+             void* stream) {
+    const Ctx& c = ctx->c;
+    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
+    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
+    REQUIRE(ct_in && ct_out, "null ciphertext");
+    REQUIRE(!vector || vw, "null plaintext table");
+    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
+    Plan pl;
+    if (validate(c, level, prog, pl, vw)) return -1;
+    if (bgv && bgv_program_checks(*prog, pl, scale_invariant)) return -1;
+    if (vw) {                                          // the plaintext block may not overlap the input or the output ciphertexts
+        int ptmax = 0;
+        for (int j = 0; j < vw->n_pt; j++) ptmax = std::max(ptmax, vw->pt_levels[j]);
+        const size_t ptb = ((size_t)(vw->n_pt - 1) * vw->pt_stride + (size_t)(ptmax + 1) * c.N) * 8;
+        const size_t inb = (size_t)batch * 2 * (level + 1) * c.N * 8, outb = (size_t)batch * 2 * (pl.level[prog->out_slot] + 1) * c.N * 8;
+        REQUIRE(!overlaps(vw->pt, ptb, ct_in, inb) && !overlaps(vw->pt, ptb, ct_out, outb), "the plaintext block overlaps the input or the output");
+    }
+    GadgetCt g{};
+    if (program_rlk(c, prog, rlk, g)) return -1;
+    REQUIRE_DEVICE_AS(ctx, fn);
+    return run_program(c, level, ct_in, batch, prog, pl, g, bgv, scale_invariant == 1, ct_out, (cudaStream_t)stream, vw);
 }
 
 }  // namespace
@@ -637,70 +660,22 @@ using namespace lgpu;
 extern "C" int lgpu_ckks_polynomial_evaluate(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
                                              const lgpu_gadget_ct* rlk, uint64_t* ct_out, void* stream) {
     REQUIRE(ctx, "null context");
-    const Ctx& c = ctx->c;
-    REQUIRE(c.ring_type == 0, "polynomial evaluation is not supported on the ConjugateInvariant ring");
-    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
-    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
-    REQUIRE(ct_in && ct_out, "null ciphertext");
-    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
-    Plan pl;
-    if (validate(c, level, prog, pl)) return -1;
-    GadgetCt g{};
-    if (program_rlk(c, prog, rlk, g)) return -1;
-    REQUIRE_DEVICE(ctx);
-    return run_program(c, level, ct_in, batch, prog, pl, g, nullptr, false, ct_out, (cudaStream_t)stream);
+    REQUIRE(ctx->c.ring_type == 0, "polynomial evaluation is not supported on the ConjugateInvariant ring");
+    return evaluate(__func__, ctx, nullptr, 0, level, ct_in, batch, prog, false, nullptr, rlk, ct_out, stream);
 }
 
 extern "C" int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
                                             const lgpu_gadget_ct* rlk, int scale_invariant, uint64_t* ct_out, void* stream) {
     REQUIRE(ev, "null BGV evaluator");
     REQUIRE(scale_invariant == 0 || scale_invariant == 1, "scale_invariant must be 0 or 1");
-    const Ctx& c = ev->ctx->c;
-    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
-    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
-    REQUIRE(ct_in && ct_out, "null ciphertext");
-    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
-    Plan pl;
-    if (validate(c, level, prog, pl)) return -1;
-    if (bgv_program_checks(*prog, pl, scale_invariant)) return -1;
-    GadgetCt g{};
-    if (program_rlk(c, prog, rlk, g)) return -1;
-    REQUIRE_DEVICE(ev->ctx);
-    return run_program(c, level, ct_in, batch, prog, pl, g, &ev->s, scale_invariant == 1, ct_out, (cudaStream_t)stream);
+    return evaluate(__func__, ev->ctx, &ev->s, scale_invariant, level, ct_in, batch, prog, false, nullptr, rlk, ct_out, stream);
 }
-
-namespace lgpu {
-namespace {
-// the plaintext block may not overlap the input or the output ciphertexts
-int check_pt_block(const Ctx& c, int level, const uint64_t* ct_in, int batch, const Plan& pl, const lgpu_poly_program* prog,
-                   const lgpu_poly_pt_weights* vw, const uint64_t* ct_out) {
-    int ptmax = 0;
-    for (int j = 0; j < vw->n_pt; j++) ptmax = std::max(ptmax, vw->pt_levels[j]);
-    const size_t ptb = ((size_t)(vw->n_pt - 1) * vw->pt_stride + (size_t)(ptmax + 1) * c.N) * 8;
-    const size_t inb = (size_t)batch * 2 * (level + 1) * c.N * 8, outb = (size_t)batch * 2 * (pl.level[prog->out_slot] + 1) * c.N * 8;
-    REQUIRE(!overlaps(vw->pt, ptb, ct_in, inb) && !overlaps(vw->pt, ptb, ct_out, outb), "the plaintext block overlaps the input or the output");
-    return 0;
-}
-}  // namespace
-}  // namespace lgpu
 
 extern "C" int lgpu_ckks_polynomial_vector_evaluate(lgpu_ctx* ctx, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
                                                     const lgpu_poly_pt_weights* pts, const lgpu_gadget_ct* rlk, uint64_t* ct_out, void* stream) {
     REQUIRE(ctx, "null context");
-    const Ctx& c = ctx->c;
-    REQUIRE(c.ring_type == 0, "polynomial evaluation is not supported on the ConjugateInvariant ring");
-    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
-    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
-    REQUIRE(ct_in && ct_out, "null ciphertext");
-    REQUIRE(pts, "null plaintext table");
-    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
-    Plan pl;
-    if (validate(c, level, prog, pl, pts)) return -1;
-    if (check_pt_block(c, level, ct_in, batch, pl, prog, pts, ct_out)) return -1;
-    GadgetCt g{};
-    if (program_rlk(c, prog, rlk, g)) return -1;
-    REQUIRE_DEVICE(ctx);
-    return run_program(c, level, ct_in, batch, prog, pl, g, nullptr, false, ct_out, (cudaStream_t)stream, pts);
+    REQUIRE(ctx->c.ring_type == 0, "polynomial evaluation is not supported on the ConjugateInvariant ring");
+    return evaluate(__func__, ctx, nullptr, 0, level, ct_in, batch, prog, true, pts, rlk, ct_out, stream);
 }
 
 extern "C" int lgpu_bgv_polynomial_vector_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,
@@ -708,18 +683,5 @@ extern "C" int lgpu_bgv_polynomial_vector_evaluate(lgpu_bgv* ev, int level, cons
                                                    void* stream) {
     REQUIRE(ev, "null BGV evaluator");
     REQUIRE(scale_invariant == 0 || scale_invariant == 1, "scale_invariant must be 0 or 1");
-    const Ctx& c = ev->ctx->c;
-    REQUIRE(level >= 0 && level < c.nQ, "level out of range");
-    REQUIRE(batch >= 1 && batch <= 65535, "batch out of range");
-    REQUIRE(ct_in && ct_out, "null ciphertext");
-    REQUIRE(pts, "null plaintext table");
-    REQUIRE_ALIGNED(AL(ct_in) && AL(ct_out));
-    Plan pl;
-    if (validate(c, level, prog, pl, pts)) return -1;
-    if (bgv_program_checks(*prog, pl, scale_invariant)) return -1;
-    if (check_pt_block(c, level, ct_in, batch, pl, prog, pts, ct_out)) return -1;
-    GadgetCt g{};
-    if (program_rlk(c, prog, rlk, g)) return -1;
-    REQUIRE_DEVICE(ev->ctx);
-    return run_program(c, level, ct_in, batch, prog, pl, g, &ev->s, scale_invariant == 1, ct_out, (cudaStream_t)stream, pts);
+    return evaluate(__func__, ev->ctx, &ev->s, scale_invariant, level, ct_in, batch, prog, true, pts, rlk, ct_out, stream);
 }

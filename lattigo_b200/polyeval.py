@@ -686,14 +686,8 @@ def plan(Q: Sequence[int], level: int, scale, coeffs, basis: int, target_scale, 
          odd: bool = True, even: bool = True, roots1: Optional[Sequence[int]] = None) -> Program:
     """The device program of Evaluate(ct, bignum.NewPolynomial(basis, coeffs, .) with IsOdd = odd, IsEven = even, targetScale) for
     a ciphertext at `level` and `scale`. roots1[i]: RootsForward[1] of Q limb i (needed for non-real coefficients only)."""
-    if basis not in (MONOMIAL, CHEBYSHEV):
-        raise ValueError("basis must be MONOMIAL or CHEBYSHEV")
-    if levels_per_rescale < 1:
-        raise ValueError("levels_per_rescale must be >= 1")
-    p = _Poly(_coeffs(coeffs), basis, odd, even)
-    if p.Degree() > 255:
-        raise ValueError("degree %d > 255 is not supported" % p.Degree())
-    return _Planner(Q, levels_per_rescale, encoding_precision, roots1).evaluate(level, Fraction(scale), p, Fraction(target_scale))
+    return plan_vector(Q, level, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale, levels_per_rescale,
+                       encoding_precision, roots1=roots1)
 
 
 class Polynomial:
@@ -741,28 +735,29 @@ def _check_vector(pv: PolynomialVector, max_slots: int, slots: int):
 def plan_vector(Q: Sequence[int], level: int, scale, pv: PolynomialVector, target_scale, levels_per_rescale: int = 1,
                 encoding_precision: int = 53, log_n: int = 0, log_slots: Optional[int] = None, roots1: Optional[Sequence[int]] = None) -> Program:
     """The device program of Evaluate(ct, pv, targetScale) for a PolynomialVector. With a Mapping: every baby step in one PTLINCOMB and
-    program.plaintexts, the slot vectors to encode (values, level, scale). Without one: plan() of Value[0] (the reference's scalar
-    path), with the vector's odd / even flags. log_n: LogN of the ring (MaxSlots = 2^(LogN - 1)); log_slots: the ciphertext's LogSlots."""
-    if levels_per_rescale < 1:
-        raise ValueError("levels_per_rescale must be >= 1")
+    program.plaintexts, the slot vectors to encode (values, level, scale). Without one: the scalar program of Value[0] (the reference's
+    scalar path), with the vector's odd / even flags. log_n: LogN of the ring (MaxSlots = 2^(LogN - 1)), needed unless pv is one polynomial
+    without a Mapping; log_slots: the ciphertext's LogSlots. roots1[i]: RootsForward[1] of Q limb i (needed for non-real coefficients
+    without a Mapping only)."""
     p0 = pv.Value[0]
     if p0.basis not in (MONOMIAL, CHEBYSHEV):
         raise ValueError("basis must be MONOMIAL or CHEBYSHEV")
-    if pv.Mapping is None and len(pv.Value) == 1:
-        return plan(Q, level, scale, p0.coeffs, p0.basis, target_scale, levels_per_rescale, encoding_precision, p0.odd, p0.even, roots1)
-    if log_n < 1:
-        raise ValueError("log_n must be the ring's LogN (>= 1), got %d" % log_n)
-    max_slots = 1 << (log_n - 1)
+    if levels_per_rescale < 1:
+        raise ValueError("levels_per_rescale must be >= 1")
+    polys = [_Poly(_coeffs(q.coeffs), q.basis, q.odd, q.even) for q in pv.Value]
+    if polys[0].Degree() > 255:
+        raise ValueError("degree %d > 255 is not supported" % polys[0].Degree())
+    max_slots = 0
+    if pv.Mapping is not None or len(pv.Value) > 1:
+        if log_n < 1:
+            raise ValueError("log_n must be the ring's LogN (>= 1), got %d" % log_n)
+        max_slots = 1 << (log_n - 1)
     if pv.Mapping is not None:
         if encoding_precision > 53:
             raise ValueError("the polynomial-vector path encodes its slot vectors with the float64 encoder (EncodingPrecision <= 53); "
                              "EncodingPrecision %d is not supported" % encoding_precision)
         _check_vector(pv, max_slots, 1 << (log_n - 1 if log_slots is None else log_slots))
-    polys = [_Poly(_coeffs(q.coeffs), q.basis, q.odd, q.even) for q in pv.Value]
-    if polys[0].Degree() > 255:
-        raise ValueError("degree %d > 255 is not supported" % polys[0].Degree())
-    cplx = pv.Mapping is None and any(complex(c).imag != 0 for c in p0.coeffs)
-    if cplx and roots1 is None:
+    elif roots1 is None and any(complex(c).imag != 0 for c in p0.coeffs):
         raise ValueError("complex coefficients need the ring's RootsForward[1]")
     return _Planner(Q, levels_per_rescale, encoding_precision, roots1, max_slots).evaluate(level, Fraction(scale), polys[0], Fraction(target_scale),
                                                                                           polys[1:], pv.Mapping)
@@ -809,7 +804,35 @@ def _pt_block(ctx: Context, prog: Program, encode_group, dtype):
     return block, [prog.plaintexts[n]["level"] for n in range(len(order))]
 
 
-class PolynomialEvaluator:
+class _Evaluator:
+    """What the CKKS and BGV polynomial evaluators share. A scheme supplies plan_vector, encode_plaintexts (its encode_group) and
+    _call(level, ct, batch, prog, pts, out): its scalar entry point when pts is None, its vector entry point otherwise."""
+
+    def _prepare(self, prog: Program, pv: PolynomialVector, *encoder) -> PreparedVector:
+        """PrepareVector of a planned program: with a Mapping, its slot vectors encoded by encode_plaintexts(prog, *encoder)."""
+        pt, lv = self.encode_plaintexts(prog, *encoder) if pv.Mapping is not None else (None, [])
+        return PreparedVector(prog, pt, lv)
+
+    def _evaluate(self, ct, prep: PreparedVector):
+        return self.RunVector(prep, ct), prep.out_level, prep.out_scale
+
+    def RunVector(self, prep: PreparedVector, ct):
+        """Runs a prepared plan on ct (batch, 2, level+1, N) or (2, level+1, N). Returns the output ciphertexts."""
+        import torch
+        b = ct.shape[0] if ct.dim() == 4 else 1
+        shape = (b, 2, prep.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prep.out_level + 1, self.ctx.N)
+        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
+        self._launch(*prep.structs(self.lpr), ct, out, b)
+        return out
+
+    def run(self, prog: Program, ct, out, batch: int):
+        self._launch(prog.to_c(self.lpr), None, ct, out, batch)
+
+    def _launch(self, cp, vw, ct, out, batch: int):
+        _lib.check(self._call(ct.shape[-2] - 1, _dptr(ct), batch, ctypes.byref(cp), None if vw is None else ctypes.byref(vw), _dptr(out)))
+
+
+class PolynomialEvaluator(_Evaluator):
     """polynomial.Evaluator (circuits/ckks/polynomial) for one polynomial. encoding_precision = ckks.Parameters.EncodingPrecision()
     = max(53, log2(DefaultScale))."""
 
@@ -823,19 +846,11 @@ class PolynomialEvaluator:
         return self._roots1
 
     def plan(self, level, scale, coeffs, basis, target_scale, odd=True, even=True) -> Program:
-        cplx = any(complex(c).imag != 0 for c in coeffs)
-        return plan(self.ctx.Q, level, scale, coeffs, basis, target_scale, self.lpr, self.prec, odd, even, self.roots1() if cplx else None)
+        return self.plan_vector(level, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale)
 
     def Evaluate(self, ct, scale, coeffs, basis, target_scale, odd=True, even=True):
         """ct: (batch, 2, level+1, N) or (2, level+1, N) int64 CUDA tensor, NTT domain. Returns (ct_out, level, scale)."""
-        import torch
-        level = ct.shape[-2] - 1
-        prog = self.plan(level, scale, coeffs, basis, target_scale, odd, even)
-        b = ct.shape[0] if ct.dim() == 4 else 1
-        shape = (b, 2, prog.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prog.out_level + 1, self.ctx.N)
-        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
-        self.run(prog, ct, out, b)
-        return out, prog.out_level, prog.out_scale
+        return self.EvaluateVector(ct, scale, PolynomialVector([Polynomial(coeffs, basis, odd, even)], None), target_scale)
 
     # ---- PolynomialVector (Evaluate with a Mapping) ----------------------------------------------------------------------
     def plan_vector(self, level, scale, pv: PolynomialVector, target_scale, log_slots=None) -> Program:
@@ -862,32 +877,14 @@ class PolynomialEvaluator:
 
     def PrepareVector(self, level, scale, pv: PolynomialVector, target_scale, log_slots=None) -> PreparedVector:
         """Plans Evaluate(ct, pv, target_scale) for ciphertexts at (level, scale) and encodes its slot vectors on the device."""
-        prog = self.plan_vector(level, scale, pv, target_scale, log_slots)
-        pt, lv = self.encode_plaintexts(prog) if pv.Mapping is not None else (None, [])
-        return PreparedVector(prog, pt, lv)
-
-    def RunVector(self, prep: PreparedVector, ct):
-        """Runs a prepared plan on ct (batch, 2, level+1, N) or (2, level+1, N). Returns the output ciphertexts."""
-        import torch
-        b = ct.shape[0] if ct.dim() == 4 else 1
-        shape = (b, 2, prep.out_level + 1, self.ctx.N) if ct.dim() == 4 else (2, prep.out_level + 1, self.ctx.N)
-        out = torch.empty(shape, dtype=torch.int64, device=ct.device)
-        cp, vw = prep.structs(self.lpr)
-        if vw is None:
-            self.run(prep.prog, ct, out, b)
-        else:
-            _lib.check(_lib.lib().lgpu_ckks_polynomial_vector_evaluate(self.ctx.h, ct.shape[-2] - 1, _dptr(ct), b, ctypes.byref(cp),
-                                                                       ctypes.byref(vw), self.rlk.ref() if self.rlk is not None else None,
-                                                                       _dptr(out), _stream()))
-        return out
+        return self._prepare(self.plan_vector(level, scale, pv, target_scale, log_slots), pv)
 
     def EvaluateVector(self, ct, scale, pv: PolynomialVector, target_scale, log_slots=None):
         """Evaluate(ct, PolynomialVector, targetScale) = PrepareVector + RunVector. Returns (ct_out, level, scale)."""
-        prep = self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, log_slots)
-        return self.RunVector(prep, ct), prep.out_level, prep.out_scale
+        return self._evaluate(ct, self.PrepareVector(ct.shape[-2] - 1, scale, pv, target_scale, log_slots))
 
-    def run(self, prog: Program, ct, out, batch: int):
-        cp = prog.to_c(self.lpr)
-        _lib.check(_lib.lib().lgpu_ckks_polynomial_evaluate(self.ctx.h, ct.shape[-2] - 1, _dptr(ct), batch, ctypes.byref(cp),
-                                                            self.rlk.ref() if self.rlk is not None else None,
-                                                            _dptr(out), _stream()))
+    def _call(self, level, ct, batch, prog, pts, out):
+        rlk = self.rlk.ref() if self.rlk is not None else None
+        if pts is None:
+            return _lib.lib().lgpu_ckks_polynomial_evaluate(self.ctx.h, level, ct, batch, prog, rlk, out, _stream())
+        return _lib.lib().lgpu_ckks_polynomial_vector_evaluate(self.ctx.h, level, ct, batch, prog, pts, rlk, out, _stream())
