@@ -635,7 +635,8 @@ void lgpu_bgv_destroy(lgpu_bgv* ev);
  * evaluator.go:529-556, tensorStandard :592-667, Rescale :1363-1393), or MulRelinScaleInvariant (scale_invariant = 1, BFV;
  * :806-864, tensorScaleInvariant :898-1070; nb_rescales must be 0). ct_a, ct_b: [batch][2][level+1][N], NTT domain;
  * ct_out: [batch][2][level+1-nb_rescales][N]. ct_a == ct_b is the squaring case. ct_out == ct_a is allowed when
- * nb_rescales == 0; no other overlap. rlk: the relinearization key of ctx's (Q, P).
+ * nb_rescales == 0; no other overlap. rlk: the relinearization key of ctx's (Q, P). The scale-invariant product extends its
+ * operands from all level+1 Q moduli to QMul in one basis extension, which takes at most 64 sources: level + 1 <= 64 (BGV has no limit).
  * Scale bookkeeping stays with the caller: the reference sets the output scale to s_a * s_b (BGV), divided by q_level for
  * each Rescale, and to MulScaleInvariant(s_a, s_b, level) = s_a * s_b / (-Q_level mod t) for BFV (:983-989). */
 int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const uint64_t* ct_b, const lgpu_gadget_ct* rlk,
@@ -652,7 +653,8 @@ int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const
  *   LINCOMB  as for CKKS; the planner gives both NTT halves the same weights
  * ct_in [batch][2][level+1][N] (NTT domain) -> ct_out [batch][2][level_out+1][N]. Checked before any launch, also on a host-only
  * handle: everything lgpu_ckks_polynomial_evaluate checks, a non-null ev, scale_invariant 0 or 1, levels_per_rescale == 1, no RESCALE
- * when scale_invariant, scale-invariant MULRELIN / TENSOR operands at the op's level, and rlk at every MULRELIN / RELIN level. The
+ * when scale_invariant, scale-invariant MULRELIN / TENSOR operands at the op's level and at most 64 Q moduli (level + 1 <= 64, as for
+ * lgpu_bgv_mulrelin_batch), and rlk at every MULRELIN / RELIN level. The
  * output scale and level are the planner's. Scratch as lgpu_ckks_polynomial_evaluate, plus the QMul buffers of one
  * tensorScaleInvariant for BFV. */
 int lgpu_bgv_polynomial_evaluate(lgpu_bgv* ev, int level, const uint64_t* ct_in, int batch, const lgpu_poly_program* prog,

@@ -17,8 +17,6 @@
 
 namespace lgpu {
 
-constexpr int kMaxSrc = 64;
-
 struct ModUpParams {
     const LimbConst* limbs;
     const u64* blob;

@@ -397,6 +397,7 @@ int lgpu_bgv_mulrelin_batch(lgpu_bgv* ev, int level, const uint64_t* ct_a, const
     const Ctx& c = ev->ctx->c;
     REQUIRE(level >= 0 && level < c.nQ, "level out of range");
     REQUIRE(!scale_invariant || nb_rescales == 0, "the scale-invariant (BFV) multiplication does not rescale: nb_rescales must be 0");
+    REQUIRE(!scale_invariant || level + 1 <= kMaxSrc, "the scale-invariant (BFV) multiplication supports at most 64 Q moduli");
     REQUIRE(nb_rescales >= 0 && nb_rescales <= level, "cannot Rescale: input Ciphertext level is too low");
     const size_t N = c.N, nq = level + 1, nqo = nq - nb_rescales;
     const size_t in_bytes = (size_t)batch * 2 * nq * N * 8, out_bytes = (size_t)batch * 2 * nqo * N * 8;

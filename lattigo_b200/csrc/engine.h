@@ -20,6 +20,7 @@ typedef unsigned long long u64;
 namespace lgpu {
 
 constexpr int kMaxRows = 128;  // max limbs (rows) handled by one launch
+constexpr int kMaxSrc = 64;    // max source limbs of one basis extension (modup_kernel), so of the BFV tensor's ModUp Q -> QMul
 
 // Per-limb device constants. ring/subring.go:15-35 + ring/ntt.go:38-44.
 struct LimbConst {

@@ -583,6 +583,9 @@ int bgv_program_checks(const lgpu_poly_program& prog, const Plan& pl, int scale_
         // the scale-invariant tensor reads both operands as [batch][2][level+1][N]
         REQUIRE(!(o.kind == LGPU_POLY_MULRELIN || o.kind == LGPU_POLY_TENSOR) || (pl.level[o.src0] == o.level && pl.level[o.src1] == o.level),
                 "scale-invariant MULRELIN / TENSOR operands must be at the op's level");
+        // its operand ModUp Q -> QMul extends from all level + 1 Q moduli at once
+        REQUIRE(!(o.kind == LGPU_POLY_MULRELIN || o.kind == LGPU_POLY_TENSOR) || o.level + 1 <= kMaxSrc,
+                "the scale-invariant (BFV) multiplication supports at most 64 Q moduli");
     }
     return 0;
 }
