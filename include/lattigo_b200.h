@@ -427,6 +427,37 @@ int lgpu_encrypt_zero_sk(lgpu_ctx* ctx, int level_q, int level_p, const uint64_t
 int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t* sk_out, lgpu_gadget_ct* evk, const int64_t* e,
                             void* stream);
 
+/* ---- batched RGSW encryption and key generation at any levels (keygen.cu) -------------------------------------------------------
+ * Keys are lgpu_gadget_ct at any level_q <= max and level_p in [-1, max_p], with any BaseTwoDecomposition in [0, 62], laid out as
+ * rgsw.NewCiphertext / NewGadgetCiphertext lay them out: n_digits = BaseRNSDecompositionVectorSize(level_q, level_p), pw2_sizes =
+ * BaseTwoDecompositionVectorSize(level_q, level_p, base) (NULL when all are 1), n_pw2_max their maximum. Every key of one call has the
+ * same layout; no key's data may overlap another key or an input. The gadget factor of entry (i, j) is P_level_p 2^(base j) with
+ * P_level_p = p_0 ... p_level_p (1 when level_p = -1). sk: [nQ + nP][N] at the maximum levels, NTT + Montgomery. Secret-key
+ * encryption only, Standard ring only. Every argument check runs before any launch, also on a host-only ctx; batch and n_keys are in
+ * [1, 65535]. */
+/* rgsw.Encryptor.Encrypt (core/rgsw/encryptor.go:25-70) of batch plaintexts, or EncryptZero (:74-121) when pts == NULL. value0 /
+ * value1: HOST arrays of batch keys, Value[0] and Value[1] of each RGSW ciphertext; on entry component 1 of every entry holds its
+ * uniform polynomial (NTT domain). e: [batch][2][n_digits][n_pw2_max][N] error samples, [b][v] for Value[v] of ciphertext b.
+ * pts: [n_pt][level_q+1][N] distinct plaintexts, ciphertext b encrypting pts[pt_index[b]] (pt_index: HOST array); is_ntt /
+ * is_montgomery describe all of them and are handled as encryptor.go:47-60 does (NTT, then MForm, as needed). */
+int lgpu_rgsw_encrypt(lgpu_ctx* ctx, const uint64_t* sk, const uint64_t* pts, int n_pt, const int* pt_index, int is_ntt, int is_montgomery,
+                      const int64_t* e, const lgpu_gadget_ct* value0, const lgpu_gadget_ct* value1, int batch, void* stream);
+/* KeyGenerator.GenGaloisKeysNew(gal_els, sk, evkParams) (core/rlwe/keygenerator.go:123-209): key k encrypts sk under
+ * AutomorphismNTT(sk, gal_els[k]^-1 mod 2N). gal_els: HOST, odd and below 2N. keys: HOST array of n_keys keys, component 1 of every
+ * entry holding its uniform polynomial on entry; e: [n_keys][n_digits][n_pw2_max][N]. */
+int lgpu_gen_galois_keys(lgpu_ctx* ctx, const uint64_t* sk, const uint64_t* gal_els, int n_keys, const int64_t* e, const lgpu_gadget_ct* keys,
+                         void* stream);
+/* blindrot.GenEvaluationKeyNew (core/rgsw/blindrot/keys.go:52-108): brk0[i] / brk1[i] = Value[0] / Value[1] of RGSW(X^{s_lwe[i]}) and
+ * gks[t] the Galois key of GaloisElement(t + 1) for t < window_size, gks[window_size] that of NthRoot - GaloisGen. s_lwe: HOST array of
+ * the n_lwe (<= 32767) centred LWE-key coefficients (what the Go computes with INTT, IMForm and PolyToBigintCentered at level 0).
+ * All keys share one layout; their data is written whole. The samples are drawn here, from (seed, stream id m) for the m-th gadget
+ * ciphertext, m = 2 i + v for Value[v] of RGSW i and m = 2 n_lwe + t for gks[t]: component 1 of entry (d, j) is batch element
+ * d n_pw2_max + j of lgpu_sample_uniform(RING_Q, level_q) followed by lgpu_sample_uniform(RING_P, level_p) on that stream id, and its
+ * error is batch element d n_pw2_max + j of lgpu_sample_gaussian(sigma, bound) on it. */
+int lgpu_blind_rotation_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk, const int64_t* s_lwe, int n_lwe, int window_size, double sigma,
+                                           double bound, uint64_t seed, const lgpu_gadget_ct* brk0, const lgpu_gadget_ct* brk1,
+                                           const lgpu_gadget_ct* gks, void* stream);
+
 /* ---- threshold protocols (multiparty/), Standard ring, NTT domain ------------------------------------------------------------
  * Sampled polynomials are inputs, as for the encryptor above; every protocol's common reference polynomial comes from the same
  * samplers keyed by a seed all parties share. PublicKeyGenProtocol.GenShare (multiparty/keygen_cpk.go:70-83) is

@@ -106,6 +106,9 @@ def lib():
             "lgpu_mp_key_switch_share": [vp, i, vp, z, vp, vp, vp, vp, i, vp],
             "lgpu_mp_public_key_switch_share": [vp, i, vp, z, vp, vp, vp, vp, vp, vp, vp, i, vp],
             "lgpu_mp_evaluation_key_gen_share": [vp, vp, vp, vp, i, vp, vp, vp, vp],
+            "lgpu_rgsw_encrypt": [vp, vp, vp, i, vp, i, i, vp, vp, vp, i, vp],
+            "lgpu_gen_galois_keys": [vp, vp, vp, i, vp, vp, vp],
+            "lgpu_blind_rotation_gen_evaluation_key": [vp, vp, vp, i, i, c.c_double, c.c_double, u64, vp, vp, vp, vp],
             "lgpu_mp_rkg_share_round_one": [vp, vp, vp, vp, vp, vp, vp, vp, vp],
             "lgpu_mp_rkg_share_round_two": [vp, vp, vp, vp, vp, vp, vp],
             "lgpu_mp_shamir_share": [vp, i, i, vp, i, vp, i, vp, vp],

@@ -130,7 +130,29 @@ int sample_mask(u64 m, int n, u64 seed, u64 stream_id, u64* out, size_t bs, int 
 int sample_big_mask(int n, int W, int log_bound, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st);
 int encrypt_zero_pk(const Ctx* c, int levelQ, const u64* pk, const long long* u, const long long* e0, const long long* e1, u64* ct_out,
                     bool is_ntt, bool is_mont, int batch, cudaStream_t st);
-int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, const u64* crp, size_t crp_es, u64* evk, size_t evk_es,
-                       int n_digits, int n_pw2_max, const int* pw2_sizes, const long long* e, bool mont, cudaStream_t st);
-
+// A batch of gadget ciphertexts sharing levels and digit layout (KeyGenerator.genEvaluationKey, keygenerator.go:287-330; rgsw.Encryptor,
+// core/rgsw/encryptor.go:25-121; the multiparty key-generation shares): per ciphertext, every entry (i, j) gets
+//   component 0 = e_ij - c1_ij s_out (+ f_j pt on the Q limbs of digit i when target == 0), component 1 = c1_ij (+ f_j pt when target == 1)
+// with f_j = P_levelP 2^(pw2 j) (Montgomery form and e taken to Montgomery form when mont). Entries with j >= pw2_sizes[i] get only the
+// encryption of zero.
+struct GadgetEncLayout {
+    int levelQ, levelP, pw2, n_digits, n_pw2_max;
+    const int* pw2_sizes;     // host, per digit; nullptr = all n_pw2_max
+    size_t c0_es, c1_es;      // entry strides (words) of component 0 and of component 1 (input c1 and c1_out alike)
+    bool mont;
+};
+struct GadgetEncCt {
+    u64* c0;                  // entry (i, j) at c0 + (i n_pw2_max + j) c0_es: level_q+1 Q rows then level_p+1 P rows
+    const u64* c1;            // uniform component 1 (NTT domain), ignored when gadget_encrypt draws it
+    u64* c1_out;              // component 1 output (may equal c1); nullptr when it is neither drawn nor the target
+    const u64* s_out;         // [nQ + nP][N] secret key, NTT + Montgomery
+    u64 gal_el;               // != 0: encrypt under AutomorphismNTT(s_out, gal_el^-1 mod 2N) instead (a Galois key)
+    const u64* pt;            // rows 0..levelQ (stride N), NTT + Montgomery, or nullptr (an encryption of zero)
+    int target;               // 0 or 1
+};
+struct GadgetEncDraw { u64 seed, stream0; double sigma, bound; };   // ciphertext m draws c1 and e on stream id stream0 + m
+// e: [n_cts][n_digits][n_pw2_max][N] signed errors, or nullptr with draw != nullptr
+int gadget_encrypt(const Ctx* c, const GadgetEncLayout& g, const GadgetEncCt* cts, int n_cts, const long long* e, const GadgetEncDraw* draw,
+                   cudaStream_t st);
+int base_two_decomposition_size(const Ctx* c, int levelP, int pw2, int i);
 }  // namespace lgpu

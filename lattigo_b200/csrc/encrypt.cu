@@ -6,13 +6,17 @@
 //   Encryptor.encryptZeroSkFromC1QP / encryptZeroSk       :346-430
 //   KeyGenerator.genEvaluationKey                         core/rlwe/keygenerator.go:287-330
 //   AddPolyTimesGadgetVectorToGadgetCiphertext            core/rlwe/gadgetciphertext.go:171-241
+//   rgsw.Encryptor.Encrypt / EncryptZero                  core/rgsw/encryptor.go:25-121 (gadget_encrypt, one routine for every
+//                                                         batched gadget encryption; its C ABI is keygen.cu)
 //   ringqp.Ring.ExtendBasisSmallNormAndCenter             ring/ringqp/operations.go:325-351 (folded into small_to_rns)
 // Samplers (ring/sampler_uniform.go, sampler_ternary.go, sampler_gaussian.go): same DISTRIBUTIONS, own random streams -- the
 // reference reads a blake2b XOF sequentially (sampling/prng.go), which has no parallel form; here every coefficient owns a
 // Philox4x32-10 counter (sampler kind, seed, stream, polynomial, coefficient, attempt), so a batch of polynomials is sampled in
 // one launch and the result does not depend on the launch geometry. The layout is restated bit for bit in oracle/philox.py.
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 #include "../../include/lattigo_b200.h"
 #include "capi_common.h"
@@ -55,10 +59,22 @@ __device__ __forceinline__ Ph4 draw(const SampleKey& k, SampleKind kind, unsigne
 
 // uniform in [0, q) per row: masked 64-bit words, rejected until below q (ring/sampler_uniform.go:48-100). The polynomial index is
 // batch * kMaxRows + global limb index (P limbs are nQ + j), so the Q and P rows of one ringqp.Poly drawn on one stream id differ.
+__host__ __device__ inline SampleKey make_key(u64 seed, u64 stream) {
+    SampleKey k;
+    k.k0 = (unsigned)seed; k.k1 = (unsigned)(seed >> 32) ^ (unsigned)(stream >> 32) * 0x85EBCA6Bu; k.stream = (unsigned)stream;
+    return k;
+}
+// per_stream > 0: batch element b is element b % per_stream of stream id stream0 + b / per_stream, so one launch draws what one call
+// per stream id would (the batched key generators); per_stream = 0: every element on `key`
+struct StreamSplit { u64 seed, stream0; int per_stream; };
+__device__ __forceinline__ void split_stream(const StreamSplit& s, SampleKey& key, unsigned& b) {
+    if (s.per_stream > 0) { key = make_key(s.seed, s.stream0 + b / (unsigned)s.per_stream); b %= (unsigned)s.per_stream; }
+}
 struct UniformParams {
     const LimbConst* limbs; RowMap rm;
     u64* out; size_t rs, bs;
     SampleKey key; int n;
+    StreamSplit split;
 };
 __global__ void __launch_bounds__(256) sample_uniform_kernel(UniformParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -66,10 +82,13 @@ __global__ void __launch_bounds__(256) sample_uniform_kernel(UniformParams p) {
     const int r = blockIdx.y, b = blockIdx.z;
     const u64 q = p.limbs[p.rm.limb[r]].q;
     const u64 mask = ~0ull >> __clzll((long long)(q - 1));
-    const unsigned poly = (unsigned)b * kMaxRows + (unsigned)p.rm.limb[r];
+    SampleKey key = p.key;
+    unsigned bb = (unsigned)b;
+    split_stream(p.split, key, bb);
+    const unsigned poly = bb * kMaxRows + (unsigned)p.rm.limb[r];
     u64 v = 0;
     for (unsigned a = 0;; a++) {
-        const Ph4 d = draw(p.key, kKindUniform, poly, (unsigned)i, a);
+        const Ph4 d = draw(key, kKindUniform, poly, (unsigned)i, a);
         v = (((u64)d.x << 32) | d.y) & mask;
         if (v < q) break;
         v = (((u64)d.z << 32) | d.w) & mask;
@@ -159,12 +178,14 @@ __global__ void __launch_bounds__(256) sample_ternary_h_kernel(long long* out, i
 }
 // truncated discrete Gaussian: round(|N(0,1)| * sigma) with a random sign, redrawn while |N(0,1)| * sigma > bound
 // (ring/sampler_gaussian.go:160-182); the normal deviate comes from Box-Muller on two 53-bit uniforms
-__global__ void __launch_bounds__(256) sample_gaussian_kernel(long long* out, int n, double sigma, double bound, SampleKey key) {
+__global__ void __launch_bounds__(256) sample_gaussian_kernel(long long* out, int n, double sigma, double bound, SampleKey key, StreamSplit split) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    unsigned poly = blockIdx.y;
+    split_stream(split, key, poly);
     long long v = 0;
     for (unsigned a = 0;; a++) {
-        const Ph4 d = draw(key, kKindGaussian, blockIdx.y, (unsigned)i, a);
+        const Ph4 d = draw(key, kKindGaussian, poly, (unsigned)i, a);
         const double u1 = ((double)(((u64)d.x << 21) | (d.y >> 11)) + 1.0) * (1.0 / 9007199254740992.0);   // (0, 1]
         const double u2 = (double)(((u64)d.z << 21) | (d.w >> 11)) * (1.0 / 9007199254740992.0);            // [0, 1)
         const double z = sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
@@ -195,31 +216,76 @@ __global__ void __launch_bounds__(256) small_to_rns_kernel(SmallParams p) {
     p.out[(size_t)b * p.bs + (size_t)p.rm.drow[r] * p.rs + i] = v < 0 ? q - (u64)(-v) : (u64)v;
 }
 
-// AddPolyTimesGadgetVectorToGadgetCiphertext: evk[i][j][0][index] += pt[index] * (P w^j) on the limbs of digit i
-struct GadgetAddParams {
+// The epilogue of a batched gadget encryption (encryptZeroSkFromC1QP after its NTT, then AddPolyTimesGadgetVectorToGadgetCiphertext),
+// one word per thread pair, every row of every entry of every ciphertext of a chunk in one launch:
+//   c0 = MForm(NTT(e)) - c1 s_out   (+ f_j pt on the Q rows of digit i when the target is 0)
+//   c1 += f_j pt                    (on the Q rows of digit i when the target is 1)
+// with the word operations of the passes it replaces (LGPU_OP_MFORM, LGPU_OP_MULCOEFFSMONTGOMERYTHENSUB, CRed(c + MRed(pt, f))), so
+// its words are theirs. c0 is computed from the c1 read before the add, as the reference encrypts zero before adding the plaintext.
+struct GadgetEncDev {         // one ciphertext of the chunk (device copy of the host descriptors)
+    u64* c0;                  // entry (i, j) at c0 + (i n_pw2_max + j) c0_es
+    const u64* c1;            // entry at c1 + (.) c1_es: the uniform polynomial
+    size_t c1_es;
+    u64* c1_out;              // entry at c1_out + (.) c1_out_es; nullptr: component 1 is not written
+    const u64* s;             // [nQ + nP][N] secret of the encryption
+    const u64* pt;            // rows 0..levelQ, or nullptr
+    int target;
+};
+struct GadgetEpiParams {
     const LimbConst* limbs;
-    u64* evk; size_t ds, js;          // digit stride, pw2 stride (words); component 0 first
-    const u64* pt;                    // rows 0..levelQ, NTT + Montgomery
-    int nq, k, n, npw2;
-    const u64* f;                     // device, [index][j]: MForm(P * 2^(pw2 j) mod q_index)
+    const GadgetEncDev* cts;  // the chunk's first ciphertext
+    const u64* E;             // NTT(e) of unit u (ciphertext u / entries, entry u % entries) at E + u rows N, QP-stacked rows
+    const u64* f;             // [nq][n_pw2_max]: P_levelP 2^(pw2 j) mod q_r (Montgomery form when mont)
+    size_t c0_es, c1_out_es;
+    int nq, rows, nQ, k, n, npw2, entries, mont;
     unsigned char npw2_of_digit[kMaxRows];
 };
-__global__ void __launch_bounds__(256) gadget_add_kernel(GadgetAddParams p) {
-    const int w = blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= p.n) return;
-    const int index = blockIdx.y, j = blockIdx.z;
-    const int i = index / p.k;
-    if (j >= p.npw2_of_digit[i]) return;
-    const LimbConst& L = p.limbs[index];
-    u64* dst = p.evk + (size_t)i * p.ds + (size_t)j * p.js + (size_t)index * p.n + w;
-    const u64 t = mred(p.pt[(size_t)index * p.n + w], p.f[index * p.npw2 + j], L.q, L.qinv);
-    *dst = cred(*dst + t, L.q);
-}
-
-static SampleKey make_key(u64 seed, u64 stream) {
-    SampleKey k;
-    k.k0 = (unsigned)seed; k.k1 = (unsigned)(seed >> 32) ^ (unsigned)(stream >> 32) * 0x85EBCA6Bu; k.stream = (unsigned)stream;
-    return k;
+template <int VEC>
+__global__ void __launch_bounds__(256) gadget_enc_epilogue_kernel(GadgetEpiParams p) {
+    using V = typename std::conditional<VEC == 2, ulonglong2, u64>::type;
+    const int u = blockIdx.z, r = blockIdx.y;
+    const int b = u / p.entries, ent = u - b * p.entries;
+    const int i = ent / p.npw2, j = ent - i * p.npw2;
+    const GadgetEncDev d = p.cts[b];
+    const int limb = r < p.nq ? r : p.nQ + (r - p.nq);
+    const u64 q = p.limbs[limb].q, qinv = p.limbs[limb].qinv, bh = p.limbs[limb].bred_hi, bl = p.limbs[limb].bred_lo;
+    const size_t row = (size_t)r * p.n;
+    const V* E = reinterpret_cast<const V*>(p.E + (size_t)u * p.rows * p.n + row);
+    const V* c1 = reinterpret_cast<const V*>(d.c1 + ent * d.c1_es + row);
+    const V* s = reinterpret_cast<const V*>(d.s + (size_t)limb * p.n);
+    V* c0 = reinterpret_cast<V*>(d.c0 + ent * p.c0_es + row);
+    const bool add = d.pt && r < p.nq && r / p.k == i && j < p.npw2_of_digit[i];
+    const u64 f = add ? p.f[r * p.npw2 + j] : 0;
+    const V* pt = add ? reinterpret_cast<const V*>(d.pt + row) : nullptr;
+    const bool add0 = add && d.target == 0, add1 = add && d.target == 1;
+    V* c1o = d.c1_out ? reinterpret_cast<V*>(d.c1_out + ent * p.c1_out_es + row) : nullptr;
+    if (c1o && (const void*)c1o == (const void*)c1 && !add1) c1o = nullptr;      // component 1 unchanged in place
+    auto word = [&](u64 e, u64 a, u64 sk, u64 m, u64& o0, u64& o1) {
+        if (p.mont) e = mform(e, q, bh, bl);
+        o0 = cred(e + (q - mred(a, sk, q, qinv)), q);
+        o1 = a;
+        if (add) {
+            const u64 t = mred(m, f, q, qinv);
+            if (add0) o0 = cred(o0 + t, q);
+            else o1 = cred(a + t, q);
+        }
+    };
+    const int nv = p.n / VEC;
+    for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < nv; w += gridDim.x * blockDim.x) {
+        if constexpr (VEC == 2) {
+            const ulonglong2 e = E[w], a = c1[w], sk = s[w], m = pt ? pt[w] : make_ulonglong2(0, 0);
+            ulonglong2 o0, o1;
+            word(e.x, a.x, sk.x, m.x, o0.x, o1.x);
+            word(e.y, a.y, sk.y, m.y, o0.y, o1.y);
+            c0[w] = o0;
+            if (c1o) c1o[w] = o1;
+        } else {
+            u64 o0, o1;
+            word(E[w], c1[w], s[w], pt ? pt[w] : 0, o0, o1);
+            c0[w] = o0;
+            if (c1o) c1o[w] = o1;
+        }
+    }
 }
 
 int sample_mask(u64 m, int n, u64 seed, u64 stream_id, u64* out, size_t bs, int batch, cudaStream_t st) {
@@ -322,44 +388,106 @@ int encrypt_zero_pk(const Ctx* c, int levelQ, const u64* pk, const long long* u,
     return 0;
 }
 
-// KeyGenerator.genEvaluationKey (keygenerator.go:287-330) at the maximum levels, and the share of the multiparty protocols built on it
-// (EvaluationKeyGenProtocol.GenShare, multiparty/keygen_evk.go:86-183; component 0 of RelinearizationKeyGenProtocol.GenShareRoundOne,
-// keygen_relin.go:91-184). Entry (i, j) of evk (stride evk_es words) gets component 0 = -crp_ij sk_out + e_ij + f_j sk_in on the limbs of
-// digit i, crp entry (i, j) at stride crp_es (QP rows, NTT domain). mont: e is taken to Montgomery form and f_j = MForm(P 2^(pw2 j))
-// (key generation, EVKG); otherwise plain e and f_j = P 2^(pw2 j) (RKG round one). Entries with j >= pw2_sizes[i] are unspecified.
-int gen_evaluation_key(const Ctx* c, int pw2, const u64* sk_in, const u64* sk_out, const u64* crp, size_t crp_es, u64* evk, size_t evk_es,
-                       int n_digits, int n_pw2_max, const int* pw2_sizes, const long long* e, bool mont, cudaStream_t st) {
-    const int levelQ = c->nQ - 1, levelP = c->nP - 1;
-    const int nd = levelP >= 0 ? base_rns_decomposition_vector_size(levelQ, levelP) : levelQ + 1;
-    if (n_digits != nd) { set_error("evaluation key: n_digits != BaseRNSDecompositionVectorSize(levelQ, levelP)"); return -1; }
-    if (n_pw2_max < 1 || n_pw2_max > 64) { set_error("evaluation key: n_pw2_max out of [1, 64]"); return -1; }
-    if (pw2 < 0 || pw2 > 62) { set_error("evaluation key: BaseTwoDecomposition out of [0, 62]"); return -1; }
-    for (int i = 0; pw2_sizes && i < n_digits; i++)
-        if (pw2_sizes[i] < 1 || pw2_sizes[i] > n_pw2_max) { set_error("evaluation key: pw2_sizes[i] out of [1, n_pw2_max]"); return -1; }
-    const int entries = n_digits * n_pw2_max;
-    if (encrypt_zero_sk(c, levelQ, levelP, sk_out, const_cast<u64*>(crp), crp_es, e, evk, evk_es, true, mont, entries, st)) return -1;
-    GadgetAddParams p;
-    memset(&p, 0, sizeof(p));
-    p.limbs = c->d_limbs; p.evk = evk; p.ds = (size_t)n_pw2_max * evk_es; p.js = evk_es; p.pt = sk_in;
-    p.nq = c->nQ; p.k = levelP >= 0 ? levelP + 1 : 1; p.n = c->N; p.npw2 = n_pw2_max;
-    for (int i = 0; i < n_digits; i++) p.npw2_of_digit[i] = (unsigned char)(pw2_sizes ? pw2_sizes[i] : n_pw2_max);
-    std::vector<u64> hf((size_t)c->nQ * n_pw2_max);
-    for (int idx = 0; idx < c->nQ; idx++) {
-        const u64 q = c->Q[idx];
+// BaseTwoDecompositionVectorSize (core/rlwe/params.go:520-540) of digit i: ceil(round(log2 q_i) / pw2), or 1 when pw2 = 0 or levelP > 0
+int base_two_decomposition_size(const Ctx* c, int levelP, int pw2, int i) {
+    if (pw2 == 0 || levelP > 0) return 1;
+    const int logq = (int)std::round(std::log2((double)c->Q[i]));
+    return (logq + pw2 - 1) / pw2;
+}
+
+// Ciphertexts per chunk: LGPU_KEYGEN_CHUNK if set (read on every call), else as many as keep the chunk's scratch under 2^25 words; at
+// most 65535 entries per launch either way.
+static int keygen_chunk(size_t words_per_ct, int entries) {
+    const char* env = getenv("LGPU_KEYGEN_CHUNK");
+    long long ch = env && atoi(env) > 0 ? atoi(env) : (long long)((1ull << 25) / (words_per_ct ? words_per_ct : 1));
+    if (ch < 1) ch = 1;
+    if (ch > 65535 / entries) ch = 65535 / entries;
+    return (int)(ch < 1 ? 1 : ch);
+}
+
+int gadget_encrypt(const Ctx* c, const GadgetEncLayout& g, const GadgetEncCt* cts, int n_cts, const long long* e, const GadgetEncDraw* draw,
+                   cudaStream_t st) {
+    const size_t N = c->N;
+    const int nq = g.levelQ + 1, np = g.levelP + 1, rows = nq + np, entries = g.n_digits * g.n_pw2_max;
+    const size_t rowsN = (size_t)rows * N, key_rows = (size_t)c->nQ + c->nP;
+    const RowMap rqp = rows_qp(c, nq, np);
+    bool any_gal = false;
+    for (int b = 0; b < n_cts; b++) any_gal |= cts[b].gal_el != 0;
+    const size_t per_ct = (size_t)entries * rowsN * (draw ? 2 : 1) + (draw ? (size_t)entries * N : 0) + (any_gal ? key_rows * N : 0);
+    const int ch = keygen_chunk(per_ct, entries);
+    const int C = ch < n_cts ? ch : n_cts;
+    // f_j on the Q rows: P_levelP 2^(pw2 j) mod q (the reference's MulScalarBigint by P, then MulScalar by 2^pw2 per j)
+    std::vector<u64> hf((size_t)nq * g.n_pw2_max);
+    for (int r = 0; r < nq; r++) {
+        const u64 q = c->Q[r];
         u64 f = 1;
-        for (int j = 0; j <= levelP; j++) f = h_mulmod(f, c->P[j] % q, q);
-        for (int j = 0; j < n_pw2_max; j++) {
-            hf[(size_t)idx * n_pw2_max + j] = mont ? h_mform(f, q) : f;
-            f = h_mulmod(f, (1ull << pw2) % q, q);
+        for (int j = 0; j <= g.levelP; j++) f = h_mulmod(f, c->P[j] % q, q);
+        for (int j = 0; j < g.n_pw2_max; j++) {
+            hf[(size_t)r * g.n_pw2_max + j] = g.mont ? h_mform(f, q) : f;
+            f = h_mulmod(f, (1ull << g.pw2) % q, q);
         }
     }
-    Scratch fbuf;
+    Scratch E, U, G, S, idx, fbuf, dbuf;
+    if (E.alloc((size_t)C * entries * rowsN, st)) return -1;
+    if (draw && (U.alloc((size_t)C * entries * rowsN, st) || G.alloc((size_t)C * entries * N, st))) return -1;
+    if (any_gal && (S.alloc((size_t)C * key_rows * N, st) || idx.alloc(N, st))) return -1;
     if (fbuf.alloc(hf.size(), st)) return -1;
-    LGPU_CUDA_OK(cudaMemcpyAsync(fbuf.p, hf.data(), hf.size() * sizeof(u64), cudaMemcpyHostToDevice, st));   // pageable source: staged before return
-    p.f = fbuf.p;
-    count_launch(1);
-    gadget_add_kernel<<<dim3((c->N + 255) / 256, c->nQ, n_pw2_max), 256, 0, st>>>(p);
-    LGPU_CUDA_OK(cudaGetLastError());
+    // host descriptors: a drawn c1 lives in U, an automorphed secret in S, at the ciphertext's place in its chunk
+    std::vector<GadgetEncDev> hd((size_t)n_cts);
+    for (int b = 0; b < n_cts; b++) {
+        const GadgetEncCt& x = cts[b];
+        GadgetEncDev& dv = hd[b];
+        dv.c0 = x.c0; dv.pt = x.pt; dv.target = x.target; dv.c1_out = x.c1_out;
+        if (draw) { dv.c1 = U.p + (size_t)(b % C) * entries * rowsN; dv.c1_es = rowsN; }
+        else { dv.c1 = x.c1; dv.c1_es = g.c1_es; }
+        dv.s = x.gal_el ? S.p + (size_t)(b % C) * key_rows * N : x.s_out;
+    }
+    const size_t dwords = (hd.size() * sizeof(GadgetEncDev) + 7) / 8;
+    if (dbuf.alloc(dwords, st)) return -1;
+    // pageable sources: both copies are staged before they return
+    LGPU_CUDA_OK(cudaMemcpyAsync(fbuf.p, hf.data(), hf.size() * sizeof(u64), cudaMemcpyHostToDevice, st));
+    LGPU_CUDA_OK(cudaMemcpyAsync(dbuf.p, hd.data(), hd.size() * sizeof(GadgetEncDev), cudaMemcpyHostToDevice, st));
+    const GadgetEncDev* d_cts = reinterpret_cast<const GadgetEncDev*>(dbuf.p);
+    GadgetEpiParams p;
+    memset(&p, 0, sizeof(p));
+    p.limbs = c->d_limbs; p.E = E.p; p.f = fbuf.p; p.c0_es = g.c0_es; p.c1_out_es = g.c1_es;
+    p.nq = nq; p.rows = rows; p.nQ = c->nQ; p.k = g.levelP >= 0 ? g.levelP + 1 : 1; p.n = c->N; p.npw2 = g.n_pw2_max; p.entries = entries;
+    p.mont = g.mont ? 1 : 0;
+    for (int i = 0; i < g.n_digits; i++) p.npw2_of_digit[i] = (unsigned char)(g.pw2_sizes ? g.pw2_sizes[i] : g.n_pw2_max);
+    // 16-byte accesses when every pointer and stride allows them
+    bool vec = AL(E.p) && g.c0_es % 2 == 0 && g.c1_es % 2 == 0 && N % 2 == 0;
+    for (int b = 0; b < n_cts && vec; b++)
+        vec = AL(hd[b].c0) && AL(hd[b].c1) && hd[b].c1_es % 2 == 0 && AL(hd[b].s) && (!hd[b].pt || AL(hd[b].pt)) && (!hd[b].c1_out || AL(hd[b].c1_out));
+    const int W = vec ? 2 : 1;
+    for (int b0 = 0; b0 < n_cts; b0 += C) {
+        const int nb = n_cts - b0 < C ? n_cts - b0 : C, units = nb * entries;
+        const long long* ec = e ? e + (size_t)b0 * entries * N : (const long long*)G.p;
+        if (draw) {     // ciphertext m draws on stream id stream0 + m: the uniform c1 of entry t as batch element t, its error likewise
+            UniformParams up;
+            up.limbs = c->d_limbs; up.rm = rqp; up.out = U.p; up.rs = N; up.bs = rowsN; up.key = make_key(draw->seed, 0); up.n = c->N;
+            up.split = StreamSplit{draw->seed, draw->stream0 + (u64)b0, entries};
+            count_launch(2);
+            sample_uniform_kernel<<<dim3((c->N + 255) / 256, rows, units), 256, 0, st>>>(up);
+            sample_gaussian_kernel<<<dim3((c->N + 255) / 256, units), 256, 0, st>>>((long long*)G.p, c->N, draw->sigma, draw->bound, make_key(draw->seed, 0),
+                                                                                   StreamSplit{draw->seed, draw->stream0 + (u64)b0, entries});
+            LGPU_CUDA_OK(cudaGetLastError());
+        }
+        if (small_to_rns(c, rqp, ec, N, Span{E.p, N, rowsN}, units, st)) return -1;
+        if (launch_ntt(c, rqp, CSpan{E.p, N, rowsN}, Span{E.p, N, rowsN}, units, NTT_CANONICAL, st)) return -1;
+        for (int b = b0; b < b0 + nb; b++) {     // s_out = AutomorphismNTT(sk, galEl^-1 mod 2N) on Q and P (keygenerator.go:153-175)
+            if (!cts[b].gal_el) continue;
+            const u64 inv = h_powmod(cts[b].gal_el, (u64)c->nthroot - 1, (u64)c->nthroot);
+            if (automorphism_ntt_index(c, inv, idx.p, st)) return -1;
+            if (automorphism_ntt_with_index(c, (int)key_rows, CSpan{cts[b].s_out, N, 0}, idx.p, Span{S.p + (size_t)(b - b0) * key_rows * N, N, 0}, false, 1,
+                                            st)) return -1;
+        }
+        p.cts = d_cts + b0;
+        count_launch(1);
+        const dim3 grid((unsigned)((N / W + 255) / 256), (unsigned)rows, (unsigned)units);
+        if (vec) gadget_enc_epilogue_kernel<2><<<grid, 256, 0, st>>>(p);
+        else gadget_enc_epilogue_kernel<1><<<grid, 256, 0, st>>>(p);
+        LGPU_CUDA_OK(cudaGetLastError());
+    }
     return 0;
 }
 
@@ -375,6 +503,7 @@ int lgpu_sample_uniform(lgpu_ctx* ctx, int ring, int level, uint64_t seed, uint6
     UniformParams p;
     if (make_rowmap(ctx->c, ring, level, p.rm)) return -1;
     p.limbs = ctx->c.d_limbs; p.out = (u64*)out; p.rs = ctx->c.N; p.bs = batch_stride; p.key = make_key(seed, stream_id); p.n = ctx->c.N;
+    p.split = StreamSplit{0, 0, 0};
     count_launch(1);
     sample_uniform_kernel<<<dim3((ctx->c.N + 255) / 256, p.rm.nrows, batch), 256, 0, (cudaStream_t)stream>>>(p);
     LGPU_CUDA_OK(cudaGetLastError());
@@ -404,7 +533,8 @@ int lgpu_sample_gaussian(lgpu_ctx* ctx, double sigma, double bound, uint64_t see
     REQUIRE(sigma > 0.0 && bound >= 1.0 && bound < 9.0e18, "gaussian sampler: sigma / bound out of range");
     const int N = ctx->c.N;
     count_launch(1);
-    sample_gaussian_kernel<<<dim3((N + 255) / 256, batch), 256, 0, (cudaStream_t)stream>>>((long long*)out, N, sigma, bound, make_key(seed, stream_id));
+    sample_gaussian_kernel<<<dim3((N + 255) / 256, batch), 256, 0, (cudaStream_t)stream>>>((long long*)out, N, sigma, bound, make_key(seed, stream_id),
+                                                                                         StreamSplit{0, 0, 0});
     LGPU_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -453,8 +583,15 @@ int lgpu_gen_evaluation_key(lgpu_ctx* ctx, const uint64_t* sk_in, const uint64_t
     REQUIRE(g.levelQ == ctx->c.nQ - 1 && g.levelP == ctx->c.nP - 1, "evaluation keys are generated at the maximum levels");
     const size_t ebs = (size_t)2 * (ctx->c.nQ + ctx->c.nP) * ctx->c.N;     // component 1 of every entry holds the uniform polynomial
     u64* data = (u64*)evk->data;
-    return gen_evaluation_key(&ctx->c, g.pw2, (const u64*)sk_in, (const u64*)sk_out, data + ebs / 2, ebs, data, ebs, g.ndigits, g.npw2max, g.pw2_sizes,
-                              (const long long*)e, true, (cudaStream_t)stream);
+    const int nd = g.levelP >= 0 ? base_rns_decomposition_vector_size(g.levelQ, g.levelP) : g.levelQ + 1;
+    REQUIRE(g.ndigits == nd, "evaluation key: n_digits != BaseRNSDecompositionVectorSize(levelQ, levelP)");
+    REQUIRE(g.npw2max >= 1 && g.npw2max <= 64, "evaluation key: n_pw2_max out of [1, 64]");
+    REQUIRE(g.pw2 >= 0 && g.pw2 <= 62, "evaluation key: BaseTwoDecomposition out of [0, 62]");
+    for (int i = 0; g.pw2_sizes && i < g.ndigits; i++)
+        REQUIRE(g.pw2_sizes[i] >= 1 && g.pw2_sizes[i] <= g.npw2max, "evaluation key: pw2_sizes[i] out of [1, n_pw2_max]");
+    const GadgetEncLayout lay{g.levelQ, g.levelP, g.pw2, g.ndigits, g.npw2max, g.pw2_sizes, ebs, ebs, true};
+    const GadgetEncCt ct{data, data + ebs / 2, nullptr, (const u64*)sk_out, 0, (const u64*)sk_in, 0};
+    return gadget_encrypt(&ctx->c, lay, &ct, 1, (const long long*)e, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

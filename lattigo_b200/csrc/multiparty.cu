@@ -3,7 +3,7 @@
 //   AggregateShares (every protocol)                      e.g. multiparty/keyswitch_sk.go:123-130, keygen_cpk.go:86-89
 //   KeySwitchProtocol.GenShare, ct.IsNTT branch           multiparty/keyswitch_sk.go:85-118
 //   PublicKeySwitchProtocol.GenShare, ct.IsNTT branch     multiparty/keyswitch_pk.go:69-105
-//   EvaluationKeyGenProtocol.GenShare                     multiparty/keygen_evk.go:86-183 (gen_evaluation_key, encrypt.cu)
+//   EvaluationKeyGenProtocol.GenShare                     multiparty/keygen_evk.go:86-183 (gadget_encrypt, encrypt.cu)
 //   GaloisKeyGenProtocol.GenShare                         multiparty/keygen_gal.go:48-70
 //   RelinearizationKeyGenProtocol.GenShareRoundOne / Two  multiparty/keygen_relin.go:91-234
 //   Thresholdizer.GenShamirSecretShare, many recipients   multiparty/threshold.go:102-104
@@ -361,21 +361,13 @@ int lgpu_mp_evaluation_key_gen_share(lgpu_ctx* ctx, const uint64_t* sk_in, const
     REQUIRE(c.ring_type == 0, "multiparty key generation is not supported on the ConjugateInvariant ring");
     REQUIRE_DEVICE(ctx);
     const size_t N = c.N, rows = (size_t)c.nQ + c.nP, entries = (size_t)g.ndigits * g.npw2max, key_words = entries * rows * N;
-    cudaStream_t st = (cudaStream_t)stream;
-    Scratch buf;
-    if (gal_els && buf.alloc(rows * N + N, st)) return -1;
-    for (int k = 0; k < n_keys; k++) {
-        const u64* so = (const u64*)sk_out;
-        if (gal_els) {     // sk_out = AutomorphismNTT(sk_in, galEl^-1 mod 2N) on Q and P (keygen_gal.go:56-63)
-            const u64 inv = h_powmod(gal_els[k], (u64)c.nthroot - 1, (u64)c.nthroot);
-            if (automorphism_ntt_index(&c, inv, buf.p + rows * N, st)) return -1;
-            if (automorphism_ntt_with_index(&c, (int)rows, CSpan{(const u64*)sk_in, N, 0}, buf.p + rows * N, Span{buf.p, N, 0}, false, 1, st)) return -1;
-            so = buf.p;
-        }
-        if (gen_evaluation_key(&c, g.pw2, (const u64*)sk_in, so, (const u64*)crp + k * key_words, rows * N, (u64*)share->data + k * key_words, rows * N,
-                               g.ndigits, g.npw2max, g.pw2_sizes, (const long long*)e + k * entries * N, true, st)) return -1;
-    }
-    return 0;
+    // sk_out = AutomorphismNTT(sk_in, galEl^-1 mod 2N) on Q and P for a Galois key (keygen_gal.go:56-63)
+    std::vector<GadgetEncCt> cts((size_t)n_keys);
+    for (int k = 0; k < n_keys; k++)
+        cts[k] = GadgetEncCt{(u64*)share->data + k * key_words, (const u64*)crp + k * key_words, nullptr, gal_els ? (const u64*)sk_in : (const u64*)sk_out,
+                             gal_els ? gal_els[k] : 0, (const u64*)sk_in, 0};
+    const GadgetEncLayout lay{g.levelQ, g.levelP, g.pw2, g.ndigits, g.npw2max, g.pw2_sizes, rows * N, rows * N, true};
+    return gadget_encrypt(&c, lay, cts.data(), n_keys, (const long long*)e, nullptr, (cudaStream_t)stream);
 }
 
 int lgpu_mp_rkg_share_round_one(lgpu_ctx* ctx, const uint64_t* sk, const int64_t* u_small, const uint64_t* crp, const int64_t* e0,
@@ -399,8 +391,9 @@ int lgpu_mp_rkg_share_round_one(lgpu_ctx* ctx, const uint64_t* sk, const int64_t
     // component 0: e0 + P 2^(w j) s - u crp, plain form
     u64* data = (u64*)share->data;
     const size_t es = 2 * rows * N;
-    if (gen_evaluation_key(&c, g.pw2, (const u64*)sk, eph, (const u64*)crp, rows * N, data, es, g.ndigits, g.npw2max, g.pw2_sizes,
-                           (const long long*)e0, false, st)) return -1;
+    const GadgetEncLayout lay{g.levelQ, g.levelP, g.pw2, g.ndigits, g.npw2max, g.pw2_sizes, es, rows * N, false};
+    const GadgetEncCt ct{data, (const u64*)crp, nullptr, eph, 0, (const u64*)sk, 0};
+    if (gadget_encrypt(&c, lay, &ct, 1, (const long long*)e0, nullptr, st)) return -1;
     // component 1: NTT(e1) + s crp (MulCoeffsMontgomeryThenAdd)
     const Span c1{data + rows * N, N, es};
     if (small_to_rns(&c, rqp, (const long long*)e1, N, c1, entries, st)) return -1;

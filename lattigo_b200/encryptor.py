@@ -1,9 +1,10 @@
-"""Host-side mirror of the encryptor / key-generator inner loops and the samplers (include/lattigo_b200.h, csrc/encrypt.cu):
-rlwe.Encryptor.EncryptZero (core/rlwe/encryptor.go:170-430), rlwe.KeyGenerator.GenEvaluationKey
-(core/rlwe/keygenerator.go:261-330), ring.{Uniform,Ternary,Gaussian}Sampler."""
+"""Host-side mirror of the encryptor / key-generator inner loops and the samplers (include/lattigo_b200.h, csrc/encrypt.cu,
+csrc/keygen.cu): rlwe.Encryptor.EncryptZero (core/rlwe/encryptor.go:170-430), rlwe.KeyGenerator.GenEvaluationKey
+(core/rlwe/keygenerator.go:261-330) and GenGaloisKeysNew (:123-209), ring.{Uniform,Ternary,Gaussian}Sampler."""
 from __future__ import annotations
 
 import ctypes
+import math
 
 from . import _lib
 from .ring import Context, RING_Q, RING_P, _dptr, _stream
@@ -55,6 +56,38 @@ class Samplers:
         return out
 
 
+def gadget_layout(ctx: Context, levelQ: int, levelP: int, pw2: int):
+    """(BaseRNSDecompositionVectorSize, BaseTwoDecompositionVectorSize) of a key at these levels and base (core/rlwe/params.go:520-550)."""
+    nd = levelQ + 1 if levelP == -1 else (levelQ + levelP + 1) // (levelP + 1)
+    if pw2 == 0 or levelP > 0:
+        return nd, [1] * nd
+    return nd, [(int(round(math.log2(float(q)))) + pw2 - 1) // pw2 for q in ctx.Q[:nd]]
+
+
+def new_gadget_block(ctx: Context, n: int, levelQ: int, levelP: int, pw2: int):
+    """Room for n keys in one tensor (n, digits, pw2, 2, levelQ+1 + levelP+1, N) and the layout: (data, sizes). Every word of it is
+    written by the key generators that use it, so it is not zeroed."""
+    import torch
+    nd, sizes = gadget_layout(ctx, levelQ, levelP, pw2)
+    data = torch.empty((n, nd, max(sizes), 2, levelQ + 1 + levelP + 1, ctx.N), dtype=torch.int64, device="cuda:%d" % ctx.device)
+    return data, sizes
+
+
+def draw_gadget_samples(samplers: "Samplers", data, levelQ: int, levelP: int, sigma: float, bound: float):
+    """Uniform component 1 of every entry of the keys in `data` (new_gadget_block) and their errors (entries, N), each on one stream id."""
+    ctx = samplers.ctx
+    rows, N = levelQ + 1 + levelP + 1, ctx.N
+    entries = data.shape[0] * data.shape[1] * data.shape[2]
+    sid = samplers._sid(None)
+    base = data.data_ptr() + 8 * rows * N                       # component 1 of entry 0
+    L = _lib.lib()
+    _lib.check(L.lgpu_sample_uniform(ctx.h, RING_Q, levelQ, samplers.seed, sid, ctypes.c_void_p(base), entries, 2 * rows * N, _stream()))
+    if levelP >= 0:
+        _lib.check(L.lgpu_sample_uniform(ctx.h, RING_P, levelP, samplers.seed, sid, ctypes.c_void_p(base + 8 * (levelQ + 1) * N), entries,
+                                         2 * rows * N, _stream()))
+    return samplers.Gaussian(sigma, bound, batch=entries).view(tuple(data.shape[:3]) + (N,))
+
+
 def small_poly_to_rns(ctx: Context, small, levelQ: int, levelP: int = -1):
     """(batch, N) signed coefficients -> (batch, levelQ+1, N) [and (batch, levelP+1, N)] residues."""
     batch = small.shape[0]
@@ -90,7 +123,8 @@ class Encryptor:
 
 
 class KeyGenerator:
-    """rlwe.KeyGenerator.GenEvaluationKey at the maximum levels (core/rlwe/keygenerator.go:261-330)."""
+    """rlwe.KeyGenerator.GenEvaluationKey at the maximum levels (core/rlwe/keygenerator.go:261-330) and GenGaloisKeysNew at any levels
+    (:123-209)."""
 
     def __init__(self, ctx: Context):
         self.ctx = ctx
@@ -106,3 +140,24 @@ class KeyGenerator:
         evk = GadgetCiphertext(ctx, data, len(ctx.Q) - 1, len(ctx.P) - 1, pw2, pw2_sizes)
         _lib.check(_lib.lib().lgpu_gen_evaluation_key(ctx.h, _dptr(skIn), _dptr(skOut), evk.ref(), _dptr(e.contiguous()), _stream()))
         return evk
+
+    def GenGaloisKeysNew(self, galEls, sk, levelQ: int = None, levelP: int = None, pw2: int = 0, samplers: Samplers = None, sigma: float = 3.2,
+                         bound: float = 19.2, a=None, e=None):
+        """One Galois key per element of galEls (odd, below 2N) for sk ((nQ + nP, N), NTT + Montgomery), in one device call. The
+        samples come from `samplers`, or are given: a (n, digits, pw2, levelQ+1 + levelP+1, N) uniform, e (n, digits, pw2, N).
+        Returns the keys as a list of GadgetCiphertext in the order of galEls."""
+        import numpy as np
+        ctx = self.ctx
+        levelQ = len(ctx.Q) - 1 if levelQ is None else levelQ
+        levelP = len(ctx.P) - 1 if levelP is None else levelP
+        n = len(galEls)
+        data, sizes = new_gadget_block(ctx, n, levelQ, levelP, pw2)
+        if a is None:
+            e = draw_gadget_samples(samplers, data, levelQ, levelP, sigma, bound)
+        else:
+            data[:, :, :, 1] = a
+        keys = [GadgetCiphertext(ctx, data[k], levelQ, levelP, pw2, sizes) for k in range(n)]
+        arr = (_lib.GadgetCtStruct * n)(*[k.struct for k in keys])
+        g = np.ascontiguousarray(np.asarray(galEls, dtype=np.uint64))
+        _lib.check(_lib.lib().lgpu_gen_galois_keys(ctx.h, _dptr(sk), g.ctypes.data, n, _dptr(e.contiguous()), arr, _stream()))
+        return keys
